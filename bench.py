@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""480p frames/sec of the exemplar-colorization forward path on N B200s + correlation-kernel roofline.
+"""480p frames/sec of the exemplar-colorization forward path on N H100s + correlation-kernel roofline.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1]): one 480x854 grayscale frame + 1 exemplar, replicate-padded to the
 legal 480x864 (SURVEY.md fact 2: the reference rejects W % 16 != 0), N = 120*216 = 25920 positions.
@@ -16,11 +16,14 @@ Timed legs (own arm):
           host->device and the predicted ab device->host inside the timed region.
   roofline : every tensor-core convolution launch (the dominant kernel, ~78 % of the device time) and, as roofline_corr, the
           correlation (K7), timed with CUDA events on the launching stream in a single-stream pass inside this run;
-          achieved = algorithmic FLOPs / launch time against the measured dense-bf16 peak (burst: the pass lasts ~35 ms).
+          achieved = algorithmic FLOPs / launch time against the dense-bf16 peak (MEASURED_PEAKS.json when present, else
+          the H100 SXM data sheet's 989 TFLOP/s, which is not a measured figure).
   sustained : the `value` leg back to back for >= 2.5 s with its own clock samples.
   clip64 : BASELINE configs[2], 64 frames in N segments, exemplar prologue + NCCL broadcast inside the wall clock.
   rank_checksum : every rank colourises one common frame; the bit patterns must agree across ranks or the run aborts.
   cpu_baseline : the CPU oracle (port of the reference's PyTorch forward) on the host cores, bounded sample.
+--dump-outputs DIR: after the timed steps, the ab planes of the value leg's last step ([2, 480, 864] float32) are written
+to DIR/ab_last_step.npy; the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 Reference arm (--impl reference): the same CPU oracle timed step by step on rank 0 (the reference is pure
 Python/PyTorch and cannot travel to the GPU box; oracle/dvc_oracle.py is bit-exact with it, tests/golden/PIN_REPORT.txt).
 """
@@ -68,7 +71,7 @@ def synth_exemplar(seed=4321):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / power / throttle reasons streamed DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / power / throttle reasons streamed DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -111,19 +114,10 @@ class ClockSampler:
                 "samples": len(rows)}
 
 
-def ncu_traffic(kernel):
-    """DRAM bytes of one launch from the committed ncu --set full capture (profiles/), or None."""
-    path = os.path.join(ROOT, "profiles", "ncu_r2_traffic.json")
-    try:
-        return json.load(open(path))[kernel]["bytes"]
-    except Exception:
-        return None
-
-
 def measured_peak(window_s):
     """Dense bf16 peak to hold a kernel against: the BURST figure when the kernels were timed in a short window (the
     per-kernel leg lasts tens of milliseconds: the chip has not reached its power-limited steady state), the SUSTAINED
-    one for a window of a second or more (MEASURED_PEAKS.json; B200_PROFILING.md fallback otherwise)."""
+    one for a window of a second or more (MEASURED_PEAKS.json; the H100 SXM data sheet's dense bf16 figure otherwise)."""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     burst = window_s < 1.0
     if os.path.isfile(path):
@@ -132,7 +126,7 @@ def measured_peak(window_s):
             return float(d["bf16_tflops"]), f"measured bf16 dense, burst (MEASURED_PEAKS.json; timed window {window_s * 1e3:.0f} ms)"
         return (float(d.get("bf16_tflops_sustained", d.get("bf16_tflops"))),
                 f"measured bf16 dense, sustained (MEASURED_PEAKS.json; timed window {window_s:.1f} s)")
-    return (1700.0, "fallback burst (B200_PROFILING.md)") if burst else (1400.0, "fallback (B200_PROFILING.md: ~1.4 PFLOP/s sustained)")
+    return 989.0, "H100 SXM data sheet, dense bf16 at 700 W (not measured)"
 
 
 def pick_cpu_threads(sds):
@@ -213,7 +207,7 @@ def main():
     ap.add_argument("--corr-math", default=os.environ.get("DVC_CORR_MATH", "fp16x3"), choices=["fp32", "tf32x3", "bf16x3", "fp16x3"])
     ap.add_argument("--conv-math", default=os.environ.get("DVC_CONV_MATH", "tf32x3"), choices=["fp32", "tf32x3"])
     ap.add_argument("--tc-kc", type=int, default=int(os.environ.get("DVC_TC_KC", "1")),
-                    help="k-blocks summed in TMEM before promotion to fp32 registers (1 = parity mode)")
+                    help="k-blocks summed in the wgmma accumulators before promotion to fp32 registers (1 = parity mode)")
     ap.add_argument("--tc-kbytes", type=int, default=int(os.environ.get("DVC_TC_KBYTES", "128")), choices=[64, 128],
                     help="K bytes per pipeline stage of the conv engine (64 = twice the stages, measured slower)")
     ap.add_argument("--tc-f16", type=int, default=int(os.environ.get("DVC_TC_F16", "1")),
@@ -221,7 +215,7 @@ def main():
     ap.add_argument("--corr-screen", type=int, default=int(os.environ.get("DVC_CORR_SCREEN", "1")), choices=[0, 1],
                     help="1 = T->0 correlation as one fp16 screening pass + exact fp32 re-scoring of the candidates; 0 = exact 3-pass kernel")
     ap.add_argument("--corr-cluster", type=int, default=int(os.environ.get("DVC_CORR_CLUSTER", "2")), choices=[1, 2],
-                    help="2 = CTA pairs (tcgen05.mma.cta_group::2) in the correlation kernel, 1 = single CTAs")
+                    help="2 = 2-CTA clusters sharing the multicast reference tile in the correlation kernel, 1 = single CTAs")
     ap.add_argument("--tc-tail", type=int, default=int(os.environ.get("DVC_TC_TAIL", "0")),
                     help="1: partial last rounds of 256-channel conv launches run on 128-channel tiles; 0: off")
     ap.add_argument("--tc-splits", type=int, default=int(os.environ.get("DVC_TC_SPLITS", "1")),
@@ -231,10 +225,12 @@ def main():
     ap.add_argument("--clip-astreams", type=int, default=int(os.environ.get("DVC_CLIP_ASTREAMS", "1")), choices=[1, 2],
                     help="2: the frame-independent phase of frames t+1 and t+2 overlaps frame t's ColorVidNet (two streams)")
     ap.add_argument("--tc-cluster", type=int, default=int(os.environ.get("DVC_TC_CLUSTER", "2")), choices=[1, 2],
-                    help="2 = CTA pairs (tcgen05.mma.cta_group::2) in the conv engine, 1 = single CTAs")
+                    help="2 = 2-CTA clusters sharing the multicast weight tile in the conv engine, 1 = single CTAs")
     ap.add_argument("--cpu-sample", type=int, default=4, help="frames timed for cpu_baseline (0 = skip)")
     ap.add_argument("--sustain-s", type=float, default=2.5, help="length of the extra sustained run of the headline (0 = skip)")
     ap.add_argument("--clip-frames", type=int, default=64, help="frames of the config-3 clip (0 = skip)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the ab planes of the timed path's last step to DIR/ab_last_step.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "own" else args.warmup
 
@@ -313,6 +309,11 @@ def main():
     t_end = time.perf_counter()
     ms_dev = max_over_ranks(e0.elapsed_time(e1))
     launches = ctx.launch_count(True)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "ab_last_step.npy"), dev_out[K - 1].float().cpu().numpy())
 
     # ---------------- leg 2: end to end through the clip API with host buffers ----------------
     host_out = torch.empty(K, 2, H, W).pin_memory()
@@ -438,33 +439,28 @@ def main():
         "config": {
             "workload": WORKLOAD,
             "N_positions": N_POS,
-            "conv_math": ((f"tcgen05 {'3xFP16 on exactly scaled hi/lo planes' if args.tc_f16 else '3xTF32 operand split'}, "
-                           f"{'CTA pairs (cta_group::2)' if args.tc_cluster == 2 else 'single CTAs'}, TMEM chunk = "
+            "conv_math": ((f"wgmma {'3xFP16 on exactly scaled hi/lo planes' if args.tc_f16 else '3xTF32 operand split'}, "
+                           f"{'2-CTA clusters' if args.tc_cluster == 2 else 'single CTAs'}, accumulator chunk = "
                            f"{args.tc_kc} k-block(s) promoted to fp32 registers")
                           if args.conv_math == "tf32x3" else "fp32 CUDA-core (two-level accumulation)"),
             "corr_math": args.corr_math,
             "weights": "seeded random (dvc/synth.py), no checkpoint available",
-            "l2": "distinct frame per step; per-frame activation working set (>2 GB) exceeds the 126 MB L2",
+            "l2": "distinct frame per step; per-frame activation working set (>2 GB) exceeds the 50 MB L2",
             "exemplar_prepare_and_broadcast_ms": exemplar_ms,
         },
         "e2e": {"value": world * K / (ms_e2e * 1e-3), "unit": "frames/s", "h2d_bytes_per_step": H * W * 4,
                 "d2h_bytes_per_step": 2 * H * W * 4},
         "gpu_launches": launches,
         "clocks": clocks,
-        # dominant kernel by device time (profiles/launches_r2.md: conv_tc_kernel, all channel tiles, ~78 % of a frame; the
-        # 128-channel tile alone ~50 %: the launcher moved the quarter-resolution 256-channel layers onto it)
-        "roofline": {"kernel": "conv_tc_kernel (flat shifted GEMM on tcgen05, 3 MMA passes per product; all tensor-core convolution "
+        "roofline": {"kernel": "conv_tc_kernel (flat shifted GEMM on wgmma, 3 MMA passes per product; all tensor-core convolution "
                                "launches of a frame, channel tiles 256 / 128 / 64 listed under other_variants)",
                      "bound": "tensor",
                      "achieved": conv_all_tflops, "peak": peak, "unit": "TFLOP/s", "frac": conv_all_tflops / peak if peak else None,
-                     "traffic": ncu_traffic("conv_tc_kernel<128>"), "peak_source": peak_src,
-                     "traffic_note": "DRAM bytes (read + write) of ONE profiled launch of the 128-channel tile, the largest class by "
-                                     "device time (profiles/ncu_r2_traffic.json names the layer and its algorithmic bytes)",
+                     "peak_source": peak_src,
                      "launches_per_frame": conv_all[0] / KP, "ms_per_frame": conv_all[1] / KP,
                      "note": "sum of algorithmic FLOPs (2 x output pixels x taps x Cin x Cout) / sum of CUDA-event launch times, "
                              "single-stream pass of %d frames inside this run; the 3 MMA passes of the operand split are not "
-                             "counted, so frac is bounded by 1/3 of the dense 16-bit peak (cuBLAS itself reaches 66-76 %% of the "
-                             "nominal 2.25 PFLOP/s on this chip: MEASURED_PEAKS.json)" % KP,
+                             "counted, so frac is bounded by 1/3 of the dense 16-bit peak" % KP,
                      "other_variants": conv_detail},
         # the north-star kernel (BASELINE metric: correlation tensor-pipe fraction)
         "roofline_corr": {"kernel": (f"corr_screen_kernel + corr_rescore_kernel ({args.corr_math}, T<=2e-10: one fp16 pass locates every row's "
@@ -473,11 +469,10 @@ def main():
                                      f"corr_tc_kernel ({args.corr_math}) incl. operand split + merge"),
                           "bound": "tensor", "mma_passes": 1 if (args.corr_screen and args.corr_math == "fp16x3") else 3,
                           "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak if peak else None,
-                          "traffic": ncu_traffic("corr_tc_kernel"), "peak_source": peak_src, "launch_ms": corr_ms,
+                          "peak_source": peak_src, "launch_ms": corr_ms,
                           "note": "algorithmic 2*N*N*(256+3) FLOP per launch (the reference's matmul + softmax + matmul) over the CUDA-event "
                                   "time of the whole launch sequence; the exact kernel spends 3 MMA passes per product (ceiling 1/3 of the "
-                                  "dense 16-bit peak, 1/6 for tf32x3), the screened T->0 path one pass (ceiling 1; the shared-memory port "
-                                  "allows ~128 B/clk = one pass at full rate)"},
+                                  "dense 16-bit peak, 1/6 for tf32x3), the screened T->0 path one pass (ceiling 1)"},
         "serial_ms_per_frame": ms_serial,
         "rank_checksum": {"ok": rank_check_ok, "ranks": world,
                           "what": "bit pattern of ab for one common seeded frame, all_gather'ed and compared across ranks"},

@@ -1,6 +1,6 @@
 // Exact-fp32 convolution as a flat shifted GEMM on CUDA cores (DVC_MATH_FP32).
 //
-// This is the first correct CUDA path and stays as the on-GPU fp32 reference that the tcgen05
+// This is the first correct CUDA path and stays as the on-GPU fp32 reference that the wgmma
 // (3xTF32) engine is validated against.  Replaces nn.Conv2d + bias + ReLU/LeakyReLU (+ skip add,
 // + InstanceNorm statistics) at NonlocalNet.py:235-255,364-423 and ColorVidNet.py:96-143.
 //
@@ -17,9 +17,12 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 8;
 
-// TWO_LEVEL: every tap's Cin products are summed in a fresh accumulator that is then folded into the
-// running total, so the rounding-error chain is ~sqrt(Cin) + sqrt(taps) long instead of sqrt(9*Cin)
-// (the CPU reference's vectorised/blocked summation has a similarly short chain).
+// TWO_LEVEL: the products of every FOLD_STEPS k-steps (32 input channels of one tap, the k-block of the tensor-core
+// engine) are summed in a fresh accumulator that is then folded into the running total, so the rounding-error chain
+// is ~sqrt(32) + sqrt(9*Cin/32) long instead of sqrt(9*Cin) (the CPU reference's vectorised/blocked summation has a
+// similarly short chain).  Folding only once per tap left chains of up to 512 products, and the T = 0.01 softmax of
+// the correlation amplified the resulting feature error in the colour output beyond the reference's own fp32 noise.
+constexpr int FOLD_STEPS = 32 / BK;
 template <int BN, bool TWO_LEVEL>
 __global__ void __launch_bounds__(256) conv_gemm_simt_kernel(const ConvParams p) {
   constexpr int TN = BN / 16;
@@ -99,7 +102,8 @@ __global__ void __launch_bounds__(256) conv_gemm_simt_kernel(const ConvParams p)
         for (int j = 0; j < TN; ++j) acc[i][j] = fmaf(a[i], bb[j], acc[i][j]);
     }
     if constexpr (TWO_LEVEL) {
-      if ((it + 1) % kcs == 0) {  // end of a tap
+      const int kstep = (it + 1) % kcs;  // k-steps of the current tap done (0: the tap is complete)
+      if (kstep % FOLD_STEPS == 0) {
 #pragma unroll
         for (int i = 0; i < 8; ++i)
 #pragma unroll

@@ -1,28 +1,28 @@
-// Convolution on the 5th-generation tensor cores (tcgen05 + TMEM + TMA): DVC_MATH_TF32X3 (and its 3xFP16 default).
+// Convolution on the Hopper tensor cores (wgmma + TMA + mbarrier): DVC_MATH_TF32X3 (and its 3xFP16 default).
 //
 // Same flat shifted GEMM as conv_simt.cu (Y[p, co] = sum_tap sum_ci X[p + off(tap), ci] W[tap][ci][co] over the
 // padded pixel index p), with fp32-class accuracy from three 16/19-bit MMAs per product on hi/lo split operands
-// (x = hi + lo):  lo.hi + hi.lo + hi.hi  -> one fp32 TMEM tile.  Activations therefore live in HBM as two
+// (x = hi + lo):  lo.hi + hi.lo + hi.hi  -> one fp32 register tile.  Activations therefore live in HBM as two
 // padded-NHWC planes; weights are split once at load time.  Default operand format: fp16 planes of x * 2^e with an
 // exact power-of-two scale e (a host constant for tensors with a proven bound, else derived on the device from the
 // measured max |input| and the weights' L1 norm: dvc_internal.cuh, DynOut); tf32 planes (fp32 words) remain for
 // inputs without a known bound.
 //
-// Persistent kernel, one CTA per SM, CTA PAIRS by default (tcgen05.mma.cta_group::2 on two adjacent pixel tiles),
-// static round-robin over the (pixel-tile pair, channel tile) grid; 384 threads:
-//   warp 0       TMA producer: per (tap, 128-byte k-block) loads X_hi, X_lo [128 px x 128 B] at row offset
-//                off(tap) -- negative / past-the-end rows are zero-filled by TMA -- and W_hi, W_lo [BN(/2) x 128 B],
-//                SWIZZLE_128B, into an mbarrier ring; in a pair every CTA loads its own pixel rows and half of the
-//                channel rows, all bytes are counted on the leader's barrier.
-//   warp 1       TMEM owner + MMA issuer (leader CTA of a pair): 4 k-steps x 3 tcgen05.mma per k-block (the two cross
-//                terms of the whole k-block first, hi.hi last) into a ring of 512/BN TMEM accumulators;
-//                tcgen05.commit (multicast in a pair) frees the stage / publishes the chunk.
-//   warps 4..11  epilogue (256- / 64-channel tiles: the two warps of a lane quarter split the channels; 128-channel tile: the two
-//                warp sets take alternate tiles): every chunk (kc k-blocks) the TMEM partial sum is added to fp32 register totals with
-//                round-to-nearest adds (the TMEM accumulator truncates); then + bias, + skip addend, activation,
-//                InstanceNorm statistics (transpose-reduce in registers -> one double atomic per channel and tile),
-//                measured max |y|, masked store of the interior pixel as fp32 / tf32 planes / fp16 planes -- or the
-//                fused 1x1 + tanh tail of ColorVidNet instead of a store.
+// Persistent kernel, one CTA per SM, 2-CTA CLUSTERS by default (two adjacent pixel tiles of the same channel tile: each
+// CTA loads half of the weight tile and multicasts it to both), static round-robin over the (pixel-tile pair, channel
+// tile) grid; 384 threads:
+//   warp 0       TMA producer: per (tap, 128-byte k-block) loads X_hi, X_lo [BMT px x 128 B] at row offset off(tap) --
+//                negative / past-the-end rows are zero-filled by TMA -- and W_hi, W_lo [BN x 128 B], SWIZZLE_128B, into
+//                an mbarrier ring.
+//   warps 4..11  two consumer warpgroups.  Tile 128 px x 64 / 128 channels: each warpgroup owns 64 pixels; tile 64 px x
+//                256 channels: each owns 128 channels.  Per k-block 4 k-steps x 3 wgmma (the two cross terms of the whole
+//                k-block first, hi.hi last) into fp32 registers; every chunk (kc k-blocks) that partial sum is added to
+//                fp32 register totals with round-to-nearest adds (the tensor-core accumulation truncates); then + bias,
+//                + skip addend, activation, InstanceNorm statistics (shuffle reduction over the warp's pixels -> one
+//                double atomic per channel and tile), measured max |y|, masked store of the interior pixels as fp32 /
+//                tf32 planes / fp16 planes -- or the fused 1x1 + tanh tail of ColorVidNet instead of a store.
+// The channel tile is capped by the register file: partial sum + total of a 128 x 128 (or 64 x 256) tile take all of
+// the consumers' registers.
 // Replaces nn.Conv2d (+ReLU/LeakyReLU/skip add) at NonlocalNet.py:235-255,364-423 and ColorVidNet.py:96-143.
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -36,47 +36,48 @@ namespace dvc {
 
 namespace {
 
-constexpr int BM = 128;
+constexpr int NTHREADS = 384;  // warpgroup 0: warp 0 TMA (1-3 idle); warpgroups 1, 2: MMA + epilogue
+constexpr int CONSUMERS = 256;
 
-constexpr int NTHREADS = 384;  // warpgroup 0: warp 0 TMA, warp 1 MMA (2, 3 idle); warpgroups 1, 2: epilogue
+// Tile geometry of a channel tile BN: pixels per tile, warpgroups along the channels, wgmma N per warpgroup
+template <int BN>
+struct Geo {
+  static constexpr int WGN = BN == 256 ? 2 : 1;
+  static constexpr int BMT = 128 / WGN;
+  static constexpr int NW = BN / WGN;
+  static constexpr int R = NW / 2;  // accumulator registers per thread
+};
 
-// KBY = bytes of K per pipeline stage and operand row: 128 (SWIZZLE_128B, 32 tf32) or 64 (SWIZZLE_64B, 16 tf32).
-// A stage can be refilled only after its MMAs retire, so with S stages only S-1 refills are in flight while one
-// stage computes: at ~2.5 us TMA latency two 96 KB stages keep the tensor pipe ~60 % busy; the same shared memory
-// as four 48 KB stages hides the latency.
-// CL = 2 (CTA pair): each CTA stages only its half of the channel rows, so the same shared memory holds more stages.
-template <int BN, int KBY, int CL>
+// KBY = bytes of K per pipeline stage and operand row: 128 (SWIZZLE_128B, 32 tf32 / 64 fp16) or 64 (SWIZZLE_64B).
+// Every CTA holds the whole weight tile of a stage (in a cluster half of it arrives by the peer's multicast).
+template <int BN, int KBY>
 struct Cfg {
-  static constexpr int STAGES = (CL == 2 ? (BN == 256 ? 3 : 4) : (BN == 256 ? 2 : (BN == 128 ? 3 : 4))) * (128 / KBY);
-  static constexpr int A_BYTES = BM * KBY;
-  static constexpr int B_BYTES = (BN / CL) * KBY;
+  static constexpr int STAGES = (BN == 256 ? 2 : (BN == 128 ? 3 : 4)) * (128 / KBY);
+  static constexpr int A_BYTES = Geo<BN>::BMT * KBY;
+  static constexpr int B_BYTES = BN * KBY;
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  static constexpr int NBUF = 512 / BN;  // TMEM accumulators (2 / 4 / 8): deeper ring hides the flush round trip
-  // + barriers + statistics [4][2][BN] (one area per warp set on the narrow, ping-pong tiles)
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 512 + 8 * BN * 4 * (BN == 128 ? 2 : 1);
+  // + barriers + statistics [8 consumer warps][2][BN]
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 512 + 8 * 2 * BN * 4;
 };
 
 // Row-shared taps (RS): the three horizontal taps of a 3x3 row (two of a 2x2 phase-convolution row) read pixel rows
 // that differ by `dil` positions of the flat padded index, i.e. the SAME shared-memory tile shifted by dil rows.  One
-// activation tile of AR = 136 rows (>= 128 + 2 * dil) is loaded per (tap row, k-block) and the tcgen05 descriptors of the
-// taps start dil * 128 bytes apart: a third of the activation bytes through TMA and L2 (the weights still arrive per tap,
-// in a ring of their own).  What this buys: the shared-memory port -- 3 MMA passes re-read both operands -- is what
-// bounds the 128- and 64-channel tiles; per k-step a CTA of a pair writes 8 KB of activations + BN/2 * 64 B of weights by
-// TMA and reads 12 KB + 3 * BN/2 * 64 B by MMA in 3 * BN/2 tensor cycles (BN = 128: 156 B/clk against a 128 B/clk port);
-// with shared rows the activation writes drop to 2.8 KB (129 B/clk), BN = 256 goes from 104 to 90.
-template <int BN, int CL>
+// activation tile of AR = BMT + 8 rows is loaded per (tap row, k-block) and the wgmma descriptors of the taps start dil *
+// 128 bytes apart: a third of the activation bytes through TMA and L2 (the weights still arrive per tap, in a ring of
+// their own).
+template <int BN>
 struct CfgRS {
-  static constexpr int AR = 136;
-  static constexpr int A_TILE = AR * 128;              // one plane: 17 KB (a multiple of the 1024-byte swizzle atom)
+  static constexpr int AR = Geo<BN>::BMT + 8;
+  static constexpr int A_TILE = AR * 128;              // one plane (a multiple of the 1024-byte swizzle atom)
   static constexpr int A_STAGE = 2 * A_TILE;           // hi + lo
-  static constexpr int B_TILE = (BN / CL) * 128;
+  static constexpr int B_TILE = BN * 128;
   static constexpr int B_STAGE = 2 * B_TILE;
   static constexpr int A_STAGES = (BN == 256) ? 2 : 3;
-  static constexpr int B_STAGES = (BN == 256) ? (CL == 2 ? 4 : 2) : (BN == 128 ? (CL == 2 ? 6 : 3) : (CL == 2 ? 9 : 6));
+  static constexpr int B_STAGES = (BN == 64) ? 4 : (BN == 128 ? 3 : 2);
   static constexpr int RING_BYTES = A_STAGES * A_STAGE + B_STAGES * B_STAGE;
-  static constexpr int NBUF = 512 / BN;
-  static constexpr int SMEM_BYTES = RING_BYTES + 1024 + 512 + 8 * BN * 4 * (BN == 128 ? 2 : 1);
+  static constexpr int SMEM_BYTES = RING_BYTES + 1024 + 512 + 8 * 2 * BN * 4;
 };
+constexpr int RS_SLACK = 8;  // rows of shift a row-shared activation tile allows
 
 __device__ __forceinline__ float tf32_rna(float x) {
   uint32_t u;
@@ -84,12 +85,21 @@ __device__ __forceinline__ float tf32_rna(float x) {
   return __uint_as_float(u);
 }
 
-// CL = 2: the kernel runs as CTA pairs (cta_group::2) on adjacent pixel tiles of the same channel tile.  The 3 MMAs
-// per k-step of the operand split re-read both operands from shared memory, which makes a single CTA shared-memory
-// bound (BN = 256: 96 KB of TMA writes + 144 KB of MMA reads per 1536 tensor cycles = 156 B/clk against 128 B/clk;
-// BN = 128: 208 B/clk).  In a pair each CTA stages its own 128 pixel rows and only HALF of the channel rows; the
-// leader's tcgen05.mma.cta_group::2 computes the 256 x BN tile from both shared memories (104 / 156 B/clk).  Both
-// producers' TMA bytes are counted on the leader's full barrier; the leader's commits multicast to both CTAs.
+template <int CL>
+__device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
+  __syncwarp();
+  if (lane == 0) {
+    if (CL == 1) {
+      tc::mbar_arrive(bar);
+    } else {
+#pragma unroll
+      for (int r = 0; r < CL; ++r) tc::mbar_arrive_cluster(bar, (uint32_t)r);
+    }
+  }
+}
+
+// CL = 2: the kernel runs as 2-CTA clusters on adjacent pixel tiles of the same channel tile; each CTA loads its own
+// pixel rows and half of the weight rows, multicast into both CTAs (half the weight bytes through L2 per CTA).
 // F16: operands are fp16 hi/lo planes of x * 2^e (e static per tensor / layer, chosen from a proven bound so that
 // nothing overflows): the same 2 x 11 significant bits as the tf32 split at twice the MMA rate, half the operand
 // bytes and half as many truncating accumulations per unit of K; the epilogue multiplies by 2^-(e_x + e_w) (exact).
@@ -97,42 +107,26 @@ template <int BN, int CL, int KBY, bool F16, bool RS = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
     conv_tc_kernel(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUtensorMap tmXl,
                    const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const ConvTcParams p) {
-  using C = Cfg<BN, KBY, CL>;
-  using R = CfgRS<BN, CL>;
+  using G = Geo<BN>;
+  using C = Cfg<BN, KBY>;
+  using RC = CfgRS<BN>;
   static_assert(!RS || KBY == 128, "row-shared taps use 128-byte K blocks");
+  constexpr int BMT = G::BMT, R = G::R;
   constexpr int A_BYTES = C::A_BYTES;
-  constexpr int RING = RS ? R::RING_BYTES : C::STAGES * C::STAGE_BYTES;
-  constexpr int NFULL = RS ? (R::A_STAGES + R::B_STAGES) : C::STAGES;  // "full" barriers (then as many "empty" ones)
+  constexpr int RING = RS ? RC::RING_BYTES : C::STAGES * C::STAGE_BYTES;
+  constexpr int NFULL = RS ? (RC::A_STAGES + RC::B_STAGES) : C::STAGES;  // "full" barriers (then as many "empty" ones)
   constexpr int KE = F16 ? KBY / 2 : KBY / 4;  // K elements per stage
-  constexpr uint32_t IDESC = tc::umma_idesc(F16 ? 0u : 2u, BM * CL, BN);
-  // Epilogue organisation.  256-channel tile: the two warps of a TMEM lane quarter split the tile's channels (CPT = 128 each).
-  // 128-channel tile (PP, "ping-pong"): the two warp SETS (one warp per lane quarter each) take ALTERNATE tiles, every thread
-  // owning all 128 channels of its pixel -- while one set runs the tile epilogue (bias, activation, statistics, stores), the
-  // other already drains the chunks of the next tile.  With shared tiles the MMAs waited for a free accumulator while the
-  // previous tile was being stored (profiles/conv_layers_r2_experiments.md): +9 ... +20 % on the 128-channel layers.
-#ifdef DVC_NO_PINGPONG  // A/B builds only
-  constexpr bool PP = false;
-#else
-  constexpr bool PP = (BN == 128);  // (the 64-channel tile is 11 % slower this way: four warps drain a chunk slower than its MMAs)
-#endif
-  constexpr int CPT = PP ? BN : BN / 2;  // output channels per epilogue thread
-  constexpr int EPI_T = PP ? 128 : 256;  // threads that work on one tile's epilogue together
+  constexpr int FMT = F16 ? 2 : 0;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RING);
-  uint64_t* full = bars;          // RS: [A_STAGES] activation tiles, then [B_STAGES] weight tiles
+  uint64_t* full = bars;  // RS: [A_STAGES] activation tiles, then [B_STAGES] weight tiles
   uint64_t* empty = bars + NFULL;
-  // "accumulator full" barriers: ping-pong tiles have one bank per warp set -- a set only ever waits on the phases of its OWN
-  // tiles (an mbarrier wait carries one parity bit: a waiter that skipped phases could not tell them apart)
-  constexpr int NTF = (PP ? 2 : 1) * C::NBUF;
-  uint64_t* tfull = bars + 2 * NFULL;                  // [NTF]
-  uint64_t* tempty = bars + 2 * NFULL + NTF;           // [NBUF]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * NFULL + NTF + C::NBUF);
-  float* s_stat = reinterpret_cast<float*>(smem + RING + 512);  // [4 lane quarters][2][BN]
+  float* s_stat = reinterpret_cast<float*>(smem + RING + 512);  // [8 consumer warps][2][BN]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tiles = p.mtn ? p.mtn : (p.Mtot + BM - 1) / BM;
+  const int m_tiles = p.mtn ? p.mtn * (128 / BMT) : (p.Mtot + BMT - 1) / BMT;
   const int n_tiles = p.CoutPad / BN;
   const int crank = (CL == 2) ? (int)tc::cluster_ctarank() : 0;
   const int m_groups = (m_tiles + CL - 1) / CL;          // CL adjacent pixel tiles per work item
@@ -140,255 +134,102 @@ __global__ void __launch_bounds__(NTHREADS, 1)
   const int item0 = blockIdx.x / CL, item_stride = gridDim.x / CL;
   const int kbs = p.Cin / KE;
   const int nk = p.taps * kbs;
-  // The TMEM accumulator truncates on every tcgen05.mma; a chunk of `kc` k-blocks (12*kc accumulations) is
-  // therefore summed in TMEM from zero and then added -- with round-to-nearest fp32 adds -- to a register total
-  // by the epilogue warps (the tensor-core analogue of conv_simt.cu's two-level accumulation).
-  const int kc = p.kc * (128 / KBY);  // p.kc counts 32-element k-blocks (12 MMA accumulations each)
+  // Each wgmma accumulation truncates; a chunk of `kc` k-blocks (12*kc accumulations) is therefore summed in the
+  // accumulator registers from zero and then added -- with round-to-nearest fp32 adds -- to a register total (the
+  // tensor-core analogue of conv_simt.cu's two-level accumulation).
+  const int kc = p.kc * (128 / KBY);  // p.kc counts 128-byte k-blocks
   const int nchunks = (nk + kc - 1) / kc;
-  // Split-K against wave quantisation (e.g. 208 tiles on 148 SMs): a work item is (tile, split s of S); split s sums
-  // the chunks [nchunks*s/S, nchunks*(s+1)/S) on top of the register totals that split s-1 left in an fp32 workspace,
-  // so the accumulation order -- and every output bit -- is the same as without splitting.  Items are ordered
-  // split-major and every CTA walks its items in increasing order, so the chain of waits always ends at a split-0
-  // item that waits for nothing (all CTAs are resident: one per SM).
+  // Split-K against wave quantisation: a work item is (tile, split s of S); split s sums the chunks
+  // [nchunks*s/S, nchunks*(s+1)/S) on top of the register totals that split s-1 left in an fp32 workspace, so the
+  // accumulation order -- and every output bit -- is the same as without splitting.  Items are ordered split-major and
+  // every CTA walks its items in increasing order, so the chain of waits always ends at a split-0 item that waits for
+  // nothing (all CTAs are resident: one per SM).
   const int S = p.splits;
   const int total_work = total_items * S;
+  const int px0 = p.mt0 * 128;  // first pixel of this launch's tile range
 
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tmXh);
     tc::tma_prefetch_desc(&tmXl);
     tc::tma_prefetch_desc(&tmWh);
     tc::tma_prefetch_desc(&tmWl);
-    for (int i = 0; i < NFULL; ++i) tc::mbar_init(&full[i], 1), tc::mbar_init(&empty[i], 1);
-    for (int i = 0; i < NTF; ++i) tc::mbar_init(&tfull[i], 1);
-    for (int i = 0; i < C::NBUF; ++i) tc::mbar_init(&tempty[i], (PP ? 4 : 8) * CL);  // pair: both epilogues
+    for (int i = 0; i < NFULL; ++i) tc::mbar_init(&full[i], 1), tc::mbar_init(&empty[i], 8 * CL);  // consumer warps of the cluster
     tc::fence_barrier_init();
   }
-  if (CL == 2) tc::cluster_sync_all();  // both CTAs are resident before the pair allocation
-  if (warp == 1) {
-    if (CL == 2) {
-      tc::tmem_alloc_pair(tmem_slot, 512);
-      tc::tmem_relinquish_pair();
-    } else {
-      tc::tmem_alloc(tmem_slot, 512);
-      tc::tmem_relinquish();
-    }
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  if (CL == 2) tc::cluster_sync_all();  // the peer's barriers must be initialised before any remote arrive reaches them
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (CL == 2) tc::cluster_sync_all();  // the peer's barriers are initialised before any multicast or remote arrive reaches them
 
-  // register budget: the control warpgroup (warps 0-3) gives its registers to the two epilogue warpgroups
   if (warp < 4) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-  if (warp == 0) {
-    // ================= TMA producer =================
-    // The whole warp runs the loop convergently (so that addresses / coordinates are provably warp-uniform and live
-    // in uniform registers); one elected lane issues the instructions.
-    if constexpr (RS) {
-      // k runs over (tap row ty, k-block kb, tap column tx) with tx fastest: the activation tile of (ty, kb) serves
-      // its ntx taps; weights come per tap.  (No split-K in this mode: p.splits == 1.)
-      const int ntx = p.rs_ntx, ngroups = nk / ntx;
-      uint8_t* ringB = smem + R::A_STAGES * R::A_STAGE;
-      int as = 0, bs = 0;
-      uint32_t aph = 0, bph = 0;
-      for (int work = item0; work < total_work; work += item_stride) {
-        const int mg = work / n_tiles, nt = work - mg * n_tiles;
-        const int m0 = (p.mt0 + mg * CL + crank) * BM, n0 = nt * BN;
-        for (int g = 0; g < ngroups; ++g) {
-          const int ty = g / kbs, kb = g - ty * kbs;
-          tc::mbar_wait(&empty[as], aph ^ 1);
-          if (tc::elect_one()) {
-            uint8_t* st = smem + as * R::A_STAGE;
-            const int row = m0 + p.tap_off[ty * ntx];
-            if (CL == 1) {
-              tc::mbar_arrive_expect_tx(&full[as], R::A_STAGE);
-              tc::tma_load_2d(st, &tmXh, &full[as], kb * KE, row);
-              tc::tma_load_2d(st + R::A_TILE, &tmXl, &full[as], kb * KE, row);
-            } else {
-              if (crank == 0) tc::mbar_arrive_expect_tx(&full[as], 2 * R::A_STAGE);
-              tc::tma_load_2d_pair(st, &tmXh, &full[as], kb * KE, row);
-              tc::tma_load_2d_pair(st + R::A_TILE, &tmXl, &full[as], kb * KE, row);
-            }
-          }
-          __syncwarp();
-          if (++as == R::A_STAGES) as = 0, aph ^= 1;
-          for (int tx = 0; tx < ntx; ++tx) {
-            const int tap = ty * ntx + tx;
-            uint64_t* fb = &full[R::A_STAGES + bs];
-            tc::mbar_wait(&empty[R::A_STAGES + bs], bph ^ 1);
+    // register budget: the producer warpgroup gives its registers to the two consumer warpgroups
+    tc::setmaxnreg_dec<40>();
+    if (warp == 0) {
+      // ================= TMA producer =================
+      // The whole warp runs the loop convergently (so that addresses / coordinates are provably warp-uniform); one
+      // elected lane issues the instructions.
+      auto load_w = [&](uint8_t* st, uint64_t* fb, int kb, int wrow, int bbytes) {
+        if (CL == 1) {
+          tc::tma_load_2d(st, &tmWh, fb, kb * KE, wrow);
+          tc::tma_load_2d(st + bbytes, &tmWl, fb, kb * KE, wrow);
+        } else {  // my half of the channel rows, multicast into both CTAs
+          const int h = crank * (BN / 2);
+          tc::tma_load_2d_mc(st + h * KBY, &tmWh, fb, kb * KE, wrow + h, 3);
+          tc::tma_load_2d_mc(st + bbytes + h * KBY, &tmWl, fb, kb * KE, wrow + h, 3);
+        }
+      };
+      if constexpr (RS) {
+        // k runs over (tap row ty, k-block kb, tap column tx) with tx fastest: the activation tile of (ty, kb) serves
+        // its ntx taps; weights come per tap.  (No split-K in this mode: p.splits == 1.)
+        const int ntx = p.rs_ntx, ngroups = nk / ntx;
+        uint8_t* ringB = smem + RC::A_STAGES * RC::A_STAGE;
+        int as = 0, bs = 0;
+        uint32_t aph = 0, bph = 0;
+        for (int work = item0; work < total_work; work += item_stride) {
+          const int mg = work / n_tiles, nt = work - mg * n_tiles;
+          const int m0 = px0 + (mg * CL + crank) * BMT, n0 = nt * BN;
+          for (int g = 0; g < ngroups; ++g) {
+            const int ty = g / kbs, kb = g - ty * kbs;
+            tc::mbar_wait(&empty[as], aph ^ 1);
             if (tc::elect_one()) {
-              uint8_t* st = ringB + bs * R::B_STAGE;
-              if (CL == 1) {
-                tc::mbar_arrive_expect_tx(fb, R::B_STAGE);
-                tc::tma_load_2d(st, &tmWh, fb, kb * KE, tap * p.CoutPad + n0);
-                tc::tma_load_2d(st + R::B_TILE, &tmWl, fb, kb * KE, tap * p.CoutPad + n0);
-              } else {
-                if (crank == 0) tc::mbar_arrive_expect_tx(fb, 2 * R::B_STAGE);
-                const int hrow = crank * (BN / 2);
-                tc::tma_load_2d_pair(st, &tmWh, fb, kb * KE, tap * p.CoutPad + n0 + hrow);
-                tc::tma_load_2d_pair(st + R::B_TILE, &tmWl, fb, kb * KE, tap * p.CoutPad + n0 + hrow);
-              }
+              uint8_t* st = smem + as * RC::A_STAGE;
+              const int row = m0 + p.tap_off[ty * ntx];
+              tc::mbar_arrive_expect_tx(&full[as], RC::A_STAGE);
+              tc::tma_load_2d(st, &tmXh, &full[as], kb * KE, row);
+              tc::tma_load_2d(st + RC::A_TILE, &tmXl, &full[as], kb * KE, row);
             }
             __syncwarp();
-            if (++bs == R::B_STAGES) bs = 0, bph ^= 1;
+            if (++as == RC::A_STAGES) as = 0, aph ^= 1;
+            for (int tx = 0; tx < ntx; ++tx) {
+              const int tap = ty * ntx + tx;
+              uint64_t* fb = &full[RC::A_STAGES + bs];
+              tc::mbar_wait(&empty[RC::A_STAGES + bs], bph ^ 1);
+              if (tc::elect_one()) {
+                tc::mbar_arrive_expect_tx(fb, RC::B_STAGE);
+                load_w(ringB + bs * RC::B_STAGE, fb, kb, tap * p.CoutPad + n0, RC::B_TILE);
+              }
+              __syncwarp();
+              if (++bs == RC::B_STAGES) bs = 0, bph ^= 1;
+            }
           }
         }
-      }
-    } else {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int work = item0; work < total_work; work += item_stride) {
-        const int sp = work / total_items, item = work - sp * total_items;
-        const int mg = item / n_tiles, nt = item - mg * n_tiles;
-        const int m0 = (p.mt0 + mg * CL + crank) * BM, n0 = nt * BN;
-        const int k_lo = (nchunks * sp / S) * kc, k_hi = min((nchunks * (sp + 1) / S) * kc, nk);
-        for (int k = k_lo; k < k_hi; ++k) {
-          const int tap = k / kbs, kb = k - tap * kbs;
-          const int off = p.tap_off[tap];
-          tc::mbar_wait(&empty[stage], phase ^ 1);
-          if (tc::elect_one()) {
-            uint8_t* st = smem + stage * C::STAGE_BYTES;
-            const bool skip_lo = (p.dbg & 2) != 0;  // TIMING EXPERIMENT ONLY (wrong results): do not fetch the activation lo plane
-            if (CL == 1) {
+      } else {
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int work = item0; work < total_work; work += item_stride) {
+          const int sp = work / total_items, item = work - sp * total_items;
+          const int mg = item / n_tiles, nt = item - mg * n_tiles;
+          const int m0 = px0 + (mg * CL + crank) * BMT, n0 = nt * BN;
+          const int k_lo = (nchunks * sp / S) * kc, k_hi = min((nchunks * (sp + 1) / S) * kc, nk);
+          for (int k = k_lo; k < k_hi; ++k) {
+            const int tap = k / kbs, kb = k - tap * kbs;
+            const int off = p.tap_off[tap];
+            tc::mbar_wait(&empty[stage], phase ^ 1);
+            if (tc::elect_one()) {
+              uint8_t* st = smem + stage * C::STAGE_BYTES;
+              const bool skip_lo = (p.dbg & 2) != 0;  // TIMING EXPERIMENT ONLY (wrong results): do not fetch the activation lo plane
               tc::mbar_arrive_expect_tx(&full[stage], C::STAGE_BYTES - (skip_lo ? A_BYTES : 0));
               tc::tma_load_2d(st, &tmXh, &full[stage], kb * KE, m0 + off);
               if (!skip_lo) tc::tma_load_2d(st + A_BYTES, &tmXl, &full[stage], kb * KE, m0 + off);
-              tc::tma_load_2d(st + 2 * A_BYTES, &tmWh, &full[stage], kb * KE, tap * p.CoutPad + n0);
-              tc::tma_load_2d(st + 2 * A_BYTES + C::B_BYTES, &tmWl, &full[stage], kb * KE, tap * p.CoutPad + n0);
-            } else {  // my pixel rows and my half of the channel rows; all bytes are counted by the leader's barrier
-              if (crank == 0) tc::mbar_arrive_expect_tx(&full[stage], 2 * (C::STAGE_BYTES - (skip_lo ? A_BYTES : 0)));
-              const int hrow = crank * (BN / 2);
-              tc::tma_load_2d_pair(st, &tmXh, &full[stage], kb * KE, m0 + off);
-              if (!skip_lo) tc::tma_load_2d_pair(st + A_BYTES, &tmXl, &full[stage], kb * KE, m0 + off);
-              tc::tma_load_2d_pair(st + 2 * A_BYTES, &tmWh, &full[stage], kb * KE, tap * p.CoutPad + n0 + hrow);
-              tc::tma_load_2d_pair(st + 2 * A_BYTES + C::B_BYTES, &tmWl, &full[stage], kb * KE, tap * p.CoutPad + n0 + hrow);
-            }
-          }
-          __syncwarp();
-          if (++stage == C::STAGES) stage = 0, phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1 && (CL == 1 || crank == 0)) {
-    // ================= MMA issuer (warp-convergent loop, one elected lane issues; pair: the leader CTA only) ====
-    if constexpr (RS) {
-      const int ntx = p.rs_ntx;
-      const uint32_t ringB = tc::smem_u32(smem + R::A_STAGES * R::A_STAGE);
-      int as = 0, bs = 0;
-      uint32_t aph = 0, bph = 0, chunk_id = 0;
-      int tseq = 0;
-      for (int work = item0; work < total_work; work += item_stride, ++tseq) {
-        uint64_t* tfull_set = tfull + (PP ? (tseq & 1) * C::NBUF : 0);  // the bank of the warp set that owns this tile
-        for (int ch = 0; ch < nchunks; ++ch, ++chunk_id) {
-          const int buf = chunk_id % C::NBUF;
-          tc::mbar_wait(&tempty[buf], ((chunk_id / C::NBUF) & 1) ^ 1);
-          tc::tc_fence_after();
-          const uint32_t d = tmem_base + buf * BN;
-          const int k_end = min((ch + 1) * kc, nk);
-          for (int k = ch * kc; k < k_end; ++k) {
-            const int g = k / ntx, tx = k - g * ntx, ty = g / kbs;
-            if (tx == 0) tc::mbar_wait(&full[as], aph);  // the activation tile of this (tap row, k-block)
-            tc::mbar_wait(&full[R::A_STAGES + bs], bph);
-            tc::tc_fence_after();
-            // the tap's rows start (tap_off[tap] - tap_off[first tap of the row]) rows into the shared tile
-            // (p.dbg & 1: TIMING EXPERIMENT ONLY, wrong results -- every tap reads the tile at its aligned start)
-            const int shift = (p.dbg & 1) ? 0 : p.tap_off[ty * ntx + tx] - p.tap_off[ty * ntx];
-            const uint32_t sa = tc::smem_u32(smem + as * R::A_STAGE) + (uint32_t)shift * 128u;
-            const uint32_t sb = ringB + bs * R::B_STAGE;
-            const uint64_t bo = p.rs_base_offset ? ((uint64_t)(shift & 7) << 49) : 0ull;
-            const uint64_t dXh = tc::umma_desc_k128(sa) | bo, dXl = tc::umma_desc_k128(sa + R::A_TILE) | bo;
-            const uint64_t dWh = tc::umma_desc_k128(sb), dWl = tc::umma_desc_k128(sb + R::B_TILE);
-            if (tc::elect_one()) {
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) {
-                const uint64_t adv = (uint64_t)((kk * 32) >> 4);
-                if (CL == 1) {
-                  tc::umma_ss<!F16>(d, dXl + adv, dWh + adv, IDESC, (k > ch * kc || kk) ? 1u : 0u);
-                  tc::umma_ss<!F16>(d, dXh + adv, dWl + adv, IDESC, 1u);
-                } else {
-                  tc::umma_ss_pair<!F16>(d, dXl + adv, dWh + adv, IDESC, (k > ch * kc || kk) ? 1u : 0u);
-                  tc::umma_ss_pair<!F16>(d, dXh + adv, dWl + adv, IDESC, 1u);
-                }
-              }
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) {
-                const uint64_t adv = (uint64_t)((kk * 32) >> 4);
-                if (CL == 1)
-                  tc::umma_ss<!F16>(d, dXh + adv, dWh + adv, IDESC, 1u);
-                else
-                  tc::umma_ss_pair<!F16>(d, dXh + adv, dWh + adv, IDESC, 1u);
-              }
-              if (CL == 1) {
-                tc::umma_commit(&empty[R::A_STAGES + bs]);
-                if (tx == ntx - 1) tc::umma_commit(&empty[as]);
-                if (k == k_end - 1) tc::umma_commit(&tfull_set[buf]);
-              } else {
-                tc::umma_commit_pair_mc(&empty[R::A_STAGES + bs], 3);
-                if (tx == ntx - 1) tc::umma_commit_pair_mc(&empty[as], 3);
-                if (k == k_end - 1) tc::umma_commit_pair_mc(&tfull_set[buf], 3);
-              }
-            }
-            __syncwarp();
-            if (++bs == R::B_STAGES) bs = 0, bph ^= 1;
-            if (tx == ntx - 1 && ++as == R::A_STAGES) as = 0, aph ^= 1;
-          }
-        }
-      }
-    } else {
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t chunk_id = 0;  // global chunk counter: TMEM buffer = chunk_id % NBUF
-      int tseq = 0;
-      for (int work = item0; work < total_work; work += item_stride, ++tseq) {
-        uint64_t* tfull_set = tfull + (PP ? (tseq & 1) * C::NBUF : 0);  // the bank of the warp set that owns this tile
-        const int sp = work / total_items;
-        for (int ch = nchunks * sp / S; ch < nchunks * (sp + 1) / S; ++ch, ++chunk_id) {
-          const int buf = chunk_id % C::NBUF;
-          const uint32_t acc_phase = (chunk_id / C::NBUF) & 1;
-          tc::mbar_wait(&tempty[buf], acc_phase ^ 1);
-          tc::tc_fence_after();
-          const uint32_t d = tmem_base + buf * BN;
-          const int k_end = min((ch + 1) * kc, nk);
-          for (int k = ch * kc; k < k_end; ++k) {
-            tc::mbar_wait(&full[stage], phase);
-            tc::tc_fence_after();
-            const uint32_t sa = tc::smem_u32(smem + stage * C::STAGE_BYTES);
-            auto mkdesc = [](uint32_t a) { return KBY == 128 ? tc::umma_desc_k128(a) : tc::umma_desc_k64(a); };
-            const uint64_t dXh = mkdesc(sa), dXl = mkdesc(sa + A_BYTES);
-            const uint64_t dWh = mkdesc(sa + 2 * A_BYTES), dWl = mkdesc(sa + 2 * A_BYTES + C::B_BYTES);
-            if (tc::elect_one()) {
-              // Every accumulation truncates the accumulator at ITS current magnitude, so the two small cross
-              // terms of the whole k-block go first (while a fresh accumulator is still ~2^-11 of its final size,
-              // their truncations are negligible) and the dominant hi*hi terms last: 4 instead of 12 full-size
-              // truncations per k-block.
-#pragma unroll
-              for (int kk = 0; kk < KBY / 32; ++kk) {
-                const uint64_t adv = (uint64_t)((kk * 32) >> 4);
-                if (CL == 1) {
-                  tc::umma_ss<!F16>(d, dXl + adv, dWh + adv, IDESC, (k > ch * kc || kk) ? 1u : 0u);
-                  tc::umma_ss<!F16>(d, dXh + adv, dWl + adv, IDESC, 1u);
-                } else {
-                  tc::umma_ss_pair<!F16>(d, dXl + adv, dWh + adv, IDESC, (k > ch * kc || kk) ? 1u : 0u);
-                  tc::umma_ss_pair<!F16>(d, dXh + adv, dWl + adv, IDESC, 1u);
-                }
-              }
-#pragma unroll
-              for (int kk = 0; kk < KBY / 32; ++kk) {
-                const uint64_t adv = (uint64_t)((kk * 32) >> 4);
-                if (CL == 1)
-                  tc::umma_ss<!F16>(d, dXh + adv, dWh + adv, IDESC, 1u);
-                else
-                  tc::umma_ss_pair<!F16>(d, dXh + adv, dWh + adv, IDESC, 1u);
-              }
-              if (CL == 1) {
-                tc::umma_commit(&empty[stage]);
-                if (k == k_end - 1) tc::umma_commit(&tfull_set[buf]);
-              } else {  // release the stage to both producers, hand the accumulator to both epilogues
-                tc::umma_commit_pair_mc(&empty[stage], 3);
-                if (k == k_end - 1) tc::umma_commit_pair_mc(&tfull_set[buf], 3);
-              }
+              load_w(st + 2 * A_BYTES, &full[stage], kb, tap * p.CoutPad + n0, C::B_BYTES);
             }
             __syncwarp();
             if (++stage == C::STAGES) stage = 0, phase ^= 1;
@@ -396,25 +237,17 @@ __global__ void __launch_bounds__(NTHREADS, 1)
         }
       }
     }
-  }
   } else {
-    // ================= epilogue: 8 warps; thread = one output pixel x BN/2 channels =================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    const int q = warp & 3;                 // TMEM lane quarter this warp may read
-    const int wset = (warp - 4) >> 2;       // warp set 0 / 1
-    const int half = PP ? 0 : wset;         // shared tiles: which half of the tile's channels
-    const int etid = PP ? ((threadIdx.x - 128) & 127) : (threadIdx.x - 128);  // index among the EPI_T threads of this tile
-    float* s_stat_set = s_stat + (PP ? wset * 8 * BN : 0);                  // ping-pong: one statistics area per set
-    int tile_seq = 0;                       // tiles this CTA has walked so far (ping-pong: set = tile_seq & 1 owns it)
-    uint32_t par_mask = 0;                  // ping-pong: bit b = parity of this set's next "full" phase of accumulator b
+    // ================= consumers: wgmma into registers, then the epilogue on them =================
+    tc::setmaxnreg_inc<232>();
+    const int wg = (warp >> 2) - 1, wl = warp & 3, qd = lane & 3;
+    const int ctid = threadIdx.x - 128;            // consumer thread index
+    const int cw = warp - 4;                       // consumer warp index: statistics slot
+    const int ro = G::WGN == 1 ? wg * 64 : 0;      // this warpgroup's first pixel row of the tile
+    const int co = G::WGN == 2 ? wg * G::NW : 0;   // this warpgroup's first channel of the tile
+    const int prow = ro + wl * 16 + (lane >> 2);   // pixel row of register slot 0 (slot 1: + 8)
     const int img = p.Hp * p.Wp;
-    uint32_t chunk_id = 0;
-    auto epi_sync = [&]() {  // barrier among the threads that share this tile (named barrier 1, or 1 + set in ping-pong mode)
-      if constexpr (PP)
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + wset) : "memory");
-      else
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-    };
+    auto epi_sync = [&]() { asm volatile("bar.sync 1, 256;" ::: "memory"); };  // the 256 consumer threads
     // device-side scales (conv -> ReLU -> conv chains on fp16 planes, dvc_internal.cuh: DynOut)
     float oscale = p.out_scale, yscale = 1.f, amax = 0.f;
     if constexpr (F16) {
@@ -422,41 +255,21 @@ __global__ void __launch_bounds__(NTHREADS, 1)
       if (p.dyn.h16) {
         const int e_out = dyn_out_exponent(p.dyn);
         yscale = exp2_int(e_out);
-        if (threadIdx.x == 128 && blockIdx.x == 0) p.dyn.cell_out->e = e_out;
+        if (ctid == 0 && blockIdx.x == 0) p.dyn.cell_out->e = e_out;
       }
     }
-    for (int work = item0; work < total_work; work += item_stride, ++tile_seq) {
+    int stage = 0, as = 0, bs = 0;
+    uint32_t phase = 0, aph = 0, bph = 0;
+    float acc[R], tot[R];
+    for (int work = item0; work < total_work; work += item_stride) {
       const int sp = work / total_items, item = work - sp * total_items;
-      if (PP && (tile_seq & 1) != wset) {  // the other set's tile: only keep the chunk counter in step
-        chunk_id += (uint32_t)(nchunks * (sp + 1) / S - nchunks * sp / S);
-        continue;
-      }
       const int mg = item / n_tiles, nt = item - mg * n_tiles;
-      const int m0 = (p.mt0 + mg * CL + crank) * BM, n0 = nt * BN;
+      const int m0 = px0 + (mg * CL + crank) * BMT, n0 = nt * BN;
       const int tile_id = (mg * CL + crank) * n_tiles + nt;
-      const int pp = m0 + q * 32 + lane;
-      bool valid = pp < p.Mtot;
-      int b = 0, yo = 0, xo = 0;
-      if (valid) {
-        b = pp / img;
-        const int rem = pp - b * img;
-        const int yp = rem / p.Wp, xp = rem - yp * p.Wp;
-        const int y = yp - p.P, x = xp - p.P;
-        valid = (y >= 0 && y < p.H && x >= 0 && x < p.W);
-        if (p.stride == 2 && ((y | x) & 1)) valid = false;
-        yo = (y / p.stride) * p.oscale + p.oa, xo = (x / p.stride) * p.oscale + p.ob;
-      }
-      const size_t yoff = valid ? ((((size_t)b * p.yHp + yo + p.yP) * p.yWp + xo + p.yP) * p.yC + p.yCoff) : 0;
-      const size_t aoff = (valid && p.add) ? ((((size_t)b * p.aHp + yo + p.aP) * p.aWp + xo + p.aP) * p.aC) : 0;
-      const int b_first = min(m0, p.Mtot - 1) / img, b_last = min(m0 + BM - 1, p.Mtot - 1) / img;
-      const bool uniform_img = (b_first == b_last);
-
-      // ---- chunk sums: TMEM -> registers, fp32 round-to-nearest accumulation ----
-      float tot[CPT];
-      // workspace layout [tile][channel][pixel row]: for a fixed channel the 32 lanes of a warp touch 128 contiguous bytes
-      float* wsp = p.ws + ((size_t)tile_id * BN + half * CPT) * BM + q * 32 + lane;
+      // workspace layout [tile][register][consumer thread]: coalesced hand-over of the running totals
+      float* wsp = p.ws + (size_t)tile_id * BN * BMT + ctid;
       if (sp > 0) {
-        if (etid == 0) {
+        if (ctid == 0) {
           const int want = p.epoch * 16 + sp;
           int got;
           do {
@@ -465,70 +278,82 @@ __global__ void __launch_bounds__(NTHREADS, 1)
         }
         epi_sync();
 #pragma unroll
-        for (int j = 0; j < CPT; ++j) tot[j] = __ldcg(wsp + (size_t)j * BM);
+        for (int j = 0; j < R; ++j) tot[j] = __ldcg(wsp + (size_t)j * CONSUMERS);
       }
       const int ch_lo = nchunks * sp / S, ch_hi = nchunks * (sp + 1) / S;
-      // (Tested and not adopted: issuing the TMEM loads of NBUF / 2 consecutive chunks before one wait on the narrow tiles --
-      // 20-40 % SLOWER, 64-channel tile 123 -> 149 us on the full-resolution 64 -> 64 layer: the accumulators are released
-      // later and the register pressure of the 128-channel variant spills.)
-      {
-      for (int ch = ch_lo; ch < ch_hi; ++ch, ++chunk_id) {
-        const int buf = chunk_id % C::NBUF;
-        const uint32_t acc_phase = (chunk_id / C::NBUF) & 1;
-        if constexpr (PP) {  // my own bank: the parity of my next phase on this buffer
-          tc::mbar_wait(&tfull[wset * C::NBUF + buf], (par_mask >> buf) & 1u);
-          par_mask ^= 1u << buf;
-        } else {
-          tc::mbar_wait(&tfull[buf], acc_phase);
-        }
-        tc::tc_fence_after();
-        const uint32_t tsrc = tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN + half * CPT;
-        if constexpr (CPT >= 64) {
-#pragma unroll
-          for (int c = 0; c < CPT / 64; ++c) {  // two loads in flight per wait
-            uint32_t r0[32], r1[32];
-            __syncwarp();
-            tc::tmem_ld_32x32(tsrc + c * 64, r0);
-            tc::tmem_ld_32x32(tsrc + c * 64 + 32, r1);
-            tc::tmem_ld_wait();
-            if (ch == 0) {  // first chunk of the tile (always in split 0)
-#pragma unroll
-              for (int j = 0; j < 32; ++j) tot[c * 64 + j] = __uint_as_float(r0[j]), tot[c * 64 + 32 + j] = __uint_as_float(r1[j]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) tot[c * 64 + j] += __uint_as_float(r0[j]), tot[c * 64 + 32 + j] += __uint_as_float(r1[j]);
-            }
-          }
-        } else {
-          uint32_t r[32];
-          __syncwarp();
-          tc::tmem_ld_32x32(tsrc, r);
-          tc::tmem_ld_wait();
-          if (ch == 0) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) tot[j] = __uint_as_float(r[j]);
+      for (int ch = ch_lo; ch < ch_hi; ++ch) {
+        const int k_end = min((ch + 1) * kc, nk);
+        for (int k = ch * kc; k < k_end; ++k) {
+          uint32_t sa, sb;
+          uint64_t bo = 0;
+          int tx = 0, ntx = 1;
+          if constexpr (RS) {
+            ntx = p.rs_ntx;
+            const int g = k / ntx, ty = g / kbs;
+            tx = k - g * ntx;
+            if (tx == 0) tc::mbar_wait(&full[as], aph);  // the activation tile of this (tap row, k-block)
+            tc::mbar_wait(&full[RC::A_STAGES + bs], bph);
+            // the tap's rows start (tap_off[tap] - tap_off[first tap of the row]) rows into the shared tile
+            // (p.dbg & 1: TIMING EXPERIMENT ONLY, wrong results -- every tap reads the tile at its aligned start)
+            const int shift = (p.dbg & 1) ? 0 : p.tap_off[ty * ntx + tx] - p.tap_off[ty * ntx];
+            sa = tc::smem_u32(smem + as * RC::A_STAGE) + (uint32_t)(ro + shift) * 128u;
+            sb = tc::smem_u32(smem + RC::A_STAGES * RC::A_STAGE + bs * RC::B_STAGE) + (uint32_t)co * 128u;
+            bo = p.rs_base_offset ? ((uint64_t)(shift & 7) << 49) : 0ull;
           } else {
+            tc::mbar_wait(&full[stage], phase);
+            sa = tc::smem_u32(smem + stage * C::STAGE_BYTES) + (uint32_t)ro * KBY;
+            sb = tc::smem_u32(smem + stage * C::STAGE_BYTES + 2 * A_BYTES) + (uint32_t)co * KBY;
+          }
+          constexpr uint32_t A_PLANE = RS ? RC::A_TILE : A_BYTES, B_PLANE = RS ? RC::B_TILE : C::B_BYTES;
+          auto mkdesc = [](uint32_t a) { return KBY == 128 ? tc::wg_desc_k128(a) : tc::wg_desc_k64(a); };
+          const uint64_t dXh = mkdesc(sa) | bo, dXl = mkdesc(sa + A_PLANE) | bo;
+          const uint64_t dWh = mkdesc(sb), dWl = mkdesc(sb + B_PLANE);
+          tc::wg_fence_regs(acc);
+          tc::wg_fence();
+          // Every accumulation truncates the accumulator at ITS current magnitude, so the two small cross terms of the
+          // whole k-block go first (while a fresh accumulator is still ~2^-11 of its final size, their truncations are
+          // negligible) and the dominant hi*hi terms last: 4 instead of 12 full-size truncations per k-block.
 #pragma unroll
-            for (int j = 0; j < 32; ++j) tot[j] += __uint_as_float(r[j]);
+          for (int kk = 0; kk < KBY / 32; ++kk) {
+            const uint64_t adv = (uint64_t)(kk * 2);
+            tc::wgmma_fmt<FMT>(acc, dXl + adv, dWh + adv, (k > ch * kc || kk) ? 1u : 0u);
+            tc::wgmma_fmt<FMT>(acc, dXh + adv, dWl + adv, 1u);
+          }
+#pragma unroll
+          for (int kk = 0; kk < KBY / 32; ++kk) {
+            const uint64_t adv = (uint64_t)(kk * 2);
+            tc::wgmma_fmt<FMT>(acc, dXh + adv, dWh + adv, 1u);
+          }
+          tc::wg_commit();
+          tc::wg_wait<0>();
+          if constexpr (RS) {
+            release_stage<CL>(&empty[RC::A_STAGES + bs], lane);
+            if (++bs == RC::B_STAGES) bs = 0, bph ^= 1;
+            if (tx == ntx - 1) {
+              release_stage<CL>(&empty[as], lane);
+              if (++as == RC::A_STAGES) as = 0, aph ^= 1;
+            }
+          } else {
+            release_stage<CL>(&empty[stage], lane);
+            if (++stage == C::STAGES) stage = 0, phase ^= 1;
           }
         }
-        tc::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (CL == 1)
-            tc::mbar_arrive(&tempty[buf]);
-          else
-            tc::mbar_arrive_leader(&tempty[buf]);
+        tc::wg_fence_regs(acc);
+        if (ch == 0) {  // first chunk of the tile (always in split 0)
+#pragma unroll
+          for (int j = 0; j < R; ++j) tot[j] = acc[j];
+        } else {
+#pragma unroll
+          for (int j = 0; j < R; ++j) tot[j] += acc[j];
         }
       }
-      }  // CPT > 64
 
       if (sp < S - 1) {  // hand the running totals to the next split of this tile
 #pragma unroll
-        for (int j = 0; j < CPT; ++j) __stcg(wsp + (size_t)j * BM, tot[j]);
+        for (int j = 0; j < R; ++j) __stcg(wsp + (size_t)j * CONSUMERS, tot[j]);
         __threadfence();
         epi_sync();
-        if (etid == 0) {
+        if (ctid == 0) {
           const int v = p.epoch * 16 + sp + 1;
           asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p.flags + tile_id), "r"(v) : "memory");
         }
@@ -536,141 +361,132 @@ __global__ void __launch_bounds__(NTHREADS, 1)
       }
 
       // ---- bias, skip addend, activation, statistics, masked store ----
-      float fs0 = 0.f, fs1 = 0.f;  // fused 1x1 tail: partial dot products over this thread's channels
+      // register tot[4 j + 2 h + e] = pixel row prow + 8 h, channel co + 8 j + 2 qd + e
+      bool valid[2];
+      int bimg[2], yo[2], xo[2];
+      size_t yoff[2], aoff[2];
 #pragma unroll
-      for (int c = 0; c < CPT / 32; ++c) {
-        const int ch0 = n0 + half * CPT + c * 32;
-        if (ch0 < p.Cout) {
-          float v[32];
+      for (int h = 0; h < 2; ++h) {
+        const int pp = m0 + prow + 8 * h;
+        valid[h] = pp < p.Mtot;
+        bimg[h] = 0, yo[h] = 0, xo[h] = 0;
+        if (valid[h]) {
+          bimg[h] = pp / img;
+          const int rem = pp - bimg[h] * img;
+          const int yp = rem / p.Wp, xp = rem - yp * p.Wp;
+          const int y = yp - p.P, x = xp - p.P;
+          valid[h] = (y >= 0 && y < p.H && x >= 0 && x < p.W);
+          if (p.stride == 2 && ((y | x) & 1)) valid[h] = false;
+          yo[h] = (y / p.stride) * p.oscale + p.oa, xo[h] = (x / p.stride) * p.oscale + p.ob;
+        }
+        yoff[h] = valid[h] ? ((((size_t)bimg[h] * p.yHp + yo[h] + p.yP) * p.yWp + xo[h] + p.yP) * p.yC + p.yCoff) : 0;
+        aoff[h] = (valid[h] && p.add) ? ((((size_t)bimg[h] * p.aHp + yo[h] + p.aP) * p.aWp + xo[h] + p.aP) * p.aC) : 0;
+      }
+      const int b_first = min(m0, p.Mtot - 1) / img, b_last = min(m0 + BMT - 1, p.Mtot - 1) / img;
+      const bool uniform_img = (b_first == b_last);
+      float fs0[2] = {0.f, 0.f}, fs1[2] = {0.f, 0.f};  // fused 1x1 tail: partial dot products over this thread's channels
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + ch0 + j));
-            if constexpr (F16) {
-              v[j] = fmaf(tot[c * 32 + j], oscale, bv.x), v[j + 1] = fmaf(tot[c * 32 + j + 1], oscale, bv.y);
-              v[j + 2] = fmaf(tot[c * 32 + j + 2], oscale, bv.z), v[j + 3] = fmaf(tot[c * 32 + j + 3], oscale, bv.w);
-            } else {
-              v[j] = tot[c * 32 + j] + bv.x, v[j + 1] = tot[c * 32 + j + 1] + bv.y;
-              v[j + 2] = tot[c * 32 + j + 2] + bv.z, v[j + 3] = tot[c * 32 + j + 3] + bv.w;
+      for (int j = 0; j < G::NW / 8; ++j) {
+        const int chn = n0 + co + 8 * j + 2 * qd;  // channels chn, chn + 1
+        if (chn >= p.Cout) continue;
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + chn));
+        float ssum[2] = {0.f, 0.f}, ssq[2] = {0.f, 0.f};
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float v0, v1;
+          if constexpr (F16) {
+            v0 = fmaf(tot[4 * j + 2 * h], oscale, bv.x), v1 = fmaf(tot[4 * j + 2 * h + 1], oscale, bv.y);
+          } else {
+            v0 = tot[4 * j + 2 * h] + bv.x, v1 = tot[4 * j + 2 * h + 1] + bv.y;
+          }
+          if (p.add && valid[h]) {
+            float2 av = __ldg(reinterpret_cast<const float2*>(p.add + aoff[h] + chn));
+            if (p.add_lo) {
+              const float2 al = __ldg(reinterpret_cast<const float2*>(p.add_lo + aoff[h] + chn));
+              av.x += al.x, av.y += al.y;
             }
+            v0 += av.x, v1 += av.y;
           }
-          if (p.add && valid) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              float4 av = __ldg(reinterpret_cast<const float4*>(p.add + aoff + ch0 + j));
-              if (p.add_lo) {
-                const float4 al = __ldg(reinterpret_cast<const float4*>(p.add_lo + aoff + ch0 + j));
-                av.x += al.x, av.y += al.y, av.z += al.z, av.w += al.w;
-              }
-              v[j] += av.x, v[j + 1] += av.y, v[j + 2] += av.z, v[j + 3] += av.w;
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            if (p.act == ACT_RELU) v[j] = fmaxf(v[j], 0.f);
-            if (p.act == ACT_LRELU) v[j] = v[j] > 0.f ? v[j] : v[j] * p.slope;
-          }
+          if (p.act == ACT_RELU) v0 = fmaxf(v0, 0.f), v1 = fmaxf(v1, 0.f);
+          if (p.act == ACT_LRELU) v0 = v0 > 0.f ? v0 : v0 * p.slope, v1 = v1 > 0.f ? v1 : v1 * p.slope;
           if (BN == 128 && p.fin_out) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 w0 = __ldg(reinterpret_cast<const float4*>(p.fin_w + ch0 + j));
-              const float4 w1 = __ldg(reinterpret_cast<const float4*>(p.fin_w + p.Cout + ch0 + j));
-              fs0 += v[j] * w0.x + v[j + 1] * w0.y + v[j + 2] * w0.z + v[j + 3] * w0.w;
-              fs1 += v[j] * w1.x + v[j + 1] * w1.y + v[j + 2] * w1.z + v[j + 3] * w1.w;
-            }
+            const float2 w0 = __ldg(reinterpret_cast<const float2*>(p.fin_w + chn));
+            const float2 w1 = __ldg(reinterpret_cast<const float2*>(p.fin_w + p.Cout + chn));
+            fs0[h] += v0 * w0.x + v1 * w0.y;
+            fs1[h] += v0 * w1.x + v1 * w1.y;
           }
-          if (F16 && p.dyn.cell_out && valid) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) amax = fmaxf(amax, fabsf(v[j]));
-          }
-          if (valid) {
+          if (F16 && p.dyn.cell_out && valid[h]) amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+          if (valid[h]) {
             if (F16 && p.dyn.h16) {
-              __half* hp = reinterpret_cast<__half*>(p.dyn.h16) + yoff + ch0;
-              __half* lp = reinterpret_cast<__half*>(p.dyn.l16) + yoff + ch0;
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) {
-                uint32_t hw[4], lw[4];
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                  const float x0 = fminf(fmaxf(v[j + 2 * t] * yscale, -65504.f), 65504.f);
-                  const float x1 = fminf(fmaxf(v[j + 2 * t + 1] * yscale, -65504.f), 65504.f);
-                  const __half2 h2 = __floats2half2_rn(x0, x1);
-                  const float2 hf = __half22float2(h2);
-                  const __half2 l2 = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-                  hw[t] = *reinterpret_cast<const uint32_t*>(&h2), lw[t] = *reinterpret_cast<const uint32_t*>(&l2);
-                }
-                *reinterpret_cast<uint4*>(hp + j) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                *reinterpret_cast<uint4*>(lp + j) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-              }
+              const float x0 = fminf(fmaxf(v0 * yscale, -65504.f), 65504.f);
+              const float x1 = fminf(fmaxf(v1 * yscale, -65504.f), 65504.f);
+              const __half2 h2 = __floats2half2_rn(x0, x1);
+              const float2 hf = __half22float2(h2);
+              const __half2 l2 = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+              *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.dyn.h16) + yoff[h] + chn) = h2;
+              *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.dyn.l16) + yoff[h] + chn) = l2;
             } else if (p.y_lo) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                float h[4], l[4];
-#pragma unroll
-                for (int t = 0; t < 4; ++t) h[t] = tf32_rna(v[j + t]), l[t] = tf32_rna(v[j + t] - h[t]);
-                *reinterpret_cast<float4*>(p.y + yoff + ch0 + j) = make_float4(h[0], h[1], h[2], h[3]);
-                *reinterpret_cast<float4*>(p.y_lo + yoff + ch0 + j) = make_float4(l[0], l[1], l[2], l[3]);
-              }
+              const float h0 = tf32_rna(v0), h1 = tf32_rna(v1);
+              *reinterpret_cast<float2*>(p.y + yoff[h] + chn) = make_float2(h0, h1);
+              *reinterpret_cast<float2*>(p.y_lo + yoff[h] + chn) = make_float2(tf32_rna(v0 - h0), tf32_rna(v1 - h1));
             } else if (p.y) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                *reinterpret_cast<float4*>(p.y + yoff + ch0 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+              *reinterpret_cast<float2*>(p.y + yoff[h] + chn) = make_float2(v0, v1);
             }
           }
           if (p.stats) {
             if (uniform_img) {
-              // transpose-reduce: 32 channels x 32 pixels (lanes) -> lane j holds channel j's sum over the warp's
-              // pixels, in 31 shuffles per quantity (recursive halving) instead of 5 per channel; fixed order,
-              // so the statistics -- and with them the whole forward -- are run-to-run deterministic
-              float sv[32], qv[32];
-#pragma unroll
-              for (int j = 0; j < 32; ++j) sv[j] = valid ? v[j] : 0.f, qv[j] = valid ? v[j] * v[j] : 0.f;
-#pragma unroll
-              for (int off = 16, n = 16; off >= 1; off >>= 1, n >>= 1) {
-                const bool up = (lane & off) != 0;
-#pragma unroll
-                for (int i = 0; i < n; ++i) {
-                  const float send_s = up ? sv[i] : sv[i + n], keep_s = up ? sv[i + n] : sv[i];
-                  const float send_q = up ? qv[i] : qv[i + n], keep_q = up ? qv[i + n] : qv[i];
-                  sv[i] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, off);
-                  qv[i] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, off);
-                }
-              }
-              s_stat_set[(q * 2 + 0) * BN + half * CPT + c * 32 + lane] = sv[0];
-              s_stat_set[(q * 2 + 1) * BN + half * CPT + c * 32 + lane] = qv[0];
-            } else if (valid) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                atomicAdd(&p.stats[((size_t)b * p.Cout + ch0 + j) * 2 + 0], (double)v[j]);
-                atomicAdd(&p.stats[((size_t)b * p.Cout + ch0 + j) * 2 + 1], (double)v[j] * (double)v[j]);
-              }
+              if (valid[h]) ssum[0] += v0, ssum[1] += v1, ssq[0] += v0 * v0, ssq[1] += v1 * v1;
+            } else if (valid[h]) {
+              atomicAdd(&p.stats[((size_t)bimg[h] * p.Cout + chn) * 2 + 0], (double)v0);
+              atomicAdd(&p.stats[((size_t)bimg[h] * p.Cout + chn) * 2 + 1], (double)v0 * (double)v0);
+              atomicAdd(&p.stats[((size_t)bimg[h] * p.Cout + chn + 1) * 2 + 0], (double)v1);
+              atomicAdd(&p.stats[((size_t)bimg[h] * p.Cout + chn + 1) * 2 + 1], (double)v1 * (double)v1);
             }
           }
         }
+        if (p.stats && uniform_img) {
+          // the warp's 16 pixel rows of these two channels: butterfly over the 8 lanes that share qd (fixed order, so the
+          // statistics -- and with them the whole forward -- are run-to-run deterministic)
+#pragma unroll
+          for (int off = 4; off <= 16; off <<= 1) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              ssum[e] += __shfl_xor_sync(0xffffffffu, ssum[e], off);
+              ssq[e] += __shfl_xor_sync(0xffffffffu, ssq[e], off);
+            }
+          }
+          if (lane < 4) {
+            const int cl = co + 8 * j + 2 * qd;
+            s_stat[(cw * 2 + 0) * BN + cl] = ssum[0], s_stat[(cw * 2 + 0) * BN + cl + 1] = ssum[1];
+            s_stat[(cw * 2 + 1) * BN + cl] = ssq[0], s_stat[(cw * 2 + 1) * BN + cl + 1] = ssq[1];
+          }
+        }
       }
-      if (BN == 128 && p.fin_out) {  // the two channel halves of a pixel meet in shared memory
-        float2* s_fin = reinterpret_cast<float2*>(s_stat_set);
-        if (!PP) {  // shared tile: the two channel halves of a pixel meet in shared memory
-          if (half == 1) s_fin[q * 32 + lane] = make_float2(fs0, fs1);
-          epi_sync();
+      if (BN == 128 && p.fin_out) {  // a pixel's 128 channels live in the 4 threads of its quad
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int off = 1; off <= 2; off <<= 1) {
+            fs0[h] += __shfl_xor_sync(0xffffffffu, fs0[h], off);
+            fs1[h] += __shfl_xor_sync(0xffffffffu, fs1[h], off);
+          }
+          if (qd == 0 && valid[h]) {
+            const size_t hw = (size_t)p.H * p.W, po = (size_t)yo[h] * p.W + xo[h];
+            p.fin_out[((size_t)bimg[h] * 2 + 0) * hw + po] = tanhf(fs0[h] + __ldg(p.fin_b + 0)) * 128.f;
+            p.fin_out[((size_t)bimg[h] * 2 + 1) * hw + po] = tanhf(fs1[h] + __ldg(p.fin_b + 1)) * 128.f;
+          }
         }
-        if (half == 0 && valid) {
-          const float2 o2 = PP ? make_float2(0.f, 0.f) : s_fin[q * 32 + lane];
-          const size_t hw = (size_t)p.H * p.W, po = (size_t)yo * p.W + xo;
-          p.fin_out[((size_t)b * 2 + 0) * hw + po] = tanhf(fs0 + o2.x + __ldg(p.fin_b + 0)) * 128.f;
-          p.fin_out[((size_t)b * 2 + 1) * hw + po] = tanhf(fs1 + o2.y + __ldg(p.fin_b + 1)) * 128.f;
-        }
-        epi_sync();
       }
       if (p.stats) {
         epi_sync();
         if (uniform_img) {
-          for (int i = etid; i < BN; i += EPI_T) {
+          constexpr int SLOTS = 8 / G::WGN;  // consumer warps that hold partial sums of one channel
+          for (int i = ctid; i < BN; i += CONSUMERS) {
             const int chn = n0 + i;
             if (chn < p.Cout) {
-              const double s4 = (double)s_stat_set[0 * BN + i] + (double)s_stat_set[2 * BN + i] + (double)s_stat_set[4 * BN + i] +
-                                (double)s_stat_set[6 * BN + i];
-              const double q4 = (double)s_stat_set[1 * BN + i] + (double)s_stat_set[3 * BN + i] + (double)s_stat_set[5 * BN + i] +
-                                (double)s_stat_set[7 * BN + i];
+              const int w0 = G::WGN == 2 ? (i / G::NW) * 4 : 0;
+              double s4 = 0.0, q4 = 0.0;
+              for (int sl = 0; sl < SLOTS; ++sl) s4 += (double)s_stat[((w0 + sl) * 2 + 0) * BN + i], q4 += (double)s_stat[((w0 + sl) * 2 + 1) * BN + i];
               atomicAdd(&p.stats[((size_t)b_first * p.Cout + chn) * 2 + 0], s4);
               atomicAdd(&p.stats[((size_t)b_first * p.Cout + chn) * 2 + 1], q4);
             }
@@ -682,28 +498,21 @@ __global__ void __launch_bounds__(NTHREADS, 1)
     if (F16 && p.dyn.cell_out) warp_amax_commit(amax, p.dyn.cell_out);
   }
 
-  tc::tc_fence_before();
   __syncthreads();
-  if (CL == 2) tc::cluster_sync_all();  // no CTA may exit while the peer can still multicast into its shared memory
-  if (warp == 1) {
-    tc::tc_fence_after();
-    if (CL == 2)
-      tc::tmem_dealloc_pair(tmem_base, 512);
-    else
-      tc::tmem_dealloc(tmem_base, 512);
-  }
+  if (CL == 2) tc::cluster_sync_all();  // no CTA may exit while its peer can still multicast into it or arrive on its barriers
 }
 
 template <int BN, int CL, int KBY, bool F16, bool RS = false>
 int launch_bn(const CUtensorMap& mXh, const CUtensorMap& mXl, const CUtensorMap& mWh, const CUtensorMap& mWl,
               const ConvTcParams& p, int num_sms, cudaStream_t s) {
-  constexpr int SMEM = RS ? CfgRS<BN, CL>::SMEM_BYTES : Cfg<BN, KBY, CL>::SMEM_BYTES;
+  constexpr int SMEM = RS ? CfgRS<BN>::SMEM_BYTES : Cfg<BN, KBY>::SMEM_BYTES;
   static unsigned long long attr_mask = 0;  // the attribute is per device
   if (first_use_on_device(&attr_mask)) {
     if (cudaFuncSetAttribute(conv_tc_kernel<BN, CL, KBY, F16, RS>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM) != cudaSuccess)
       return -1;
   }
-  const int m_tiles = p.mtn ? p.mtn : (p.Mtot + BM - 1) / BM;
+  constexpr int BMT = Geo<BN>::BMT;
+  const int m_tiles = p.mtn ? p.mtn * (128 / BMT) : (p.Mtot + BMT - 1) / BMT;
   const int items = ((m_tiles + CL - 1) / CL) * (p.CoutPad / BN) * p.splits;
   const int max_groups = num_sms / CL;
   const int grid = CL * (items < max_groups ? items : max_groups);
@@ -720,21 +529,13 @@ int launch_bn(const CUtensorMap& mXh, const CUtensorMap& mXl, const CUtensorMap&
 
 int conv_tc_pick_bn(int cout) { return cout >= 256 ? 256 : (cout > 64 ? 128 : 64); }
 
-// Channel tile for one launch: the widest tile (best operand reuse) that still gives every SM a CTA; small
-// low-resolution layers trade tile width for parallelism.
-// The persistent grid runs ceil(items / slots) rounds, and a round costs the same whether it is full or not; a narrower
-// tile costs ~0.6x per item (measured on a B200, tools/conv_layer_bench.py: 256 -> 256 at 120x216 -- 104 pair items on 74 pair
-// slots -- takes 100 us as two rounds of 256-channel tiles and 82 us as three rounds of 128-channel tiles).
+// Channel tile for one launch: 128 channels for layers with more than 64 (the 64 x 256 tile does the same MMA work per
+// item as the 128 x 128 one but moves 320 instead of 256 operand rows per k-block, so it is only run when forced), and
+// the 64-channel tile where wider tiles would not give every SM pair a work item.
 static int pick_bn_for_launch(const ConvTcParams& p, int num_sms) {
-  const int m_tiles = (p.Mtot + BM - 1) / BM;
-  int bn = conv_tc_pick_bn(p.Cout);
+  const int m_tiles = (p.Mtot + 127) / 128;
+  int bn = conv_tc_pick_bn(p.Cout) > 128 ? 128 : conv_tc_pick_bn(p.Cout);
   while (bn > 64 && m_tiles * (p.CoutPad / bn) < num_sms / 2) bn >>= 1;
-  if (bn == 256 && p.cluster == 2 && m_tiles >= 2) {
-    const int slots = num_sms / 2, pairs = (m_tiles + 1) / 2;
-    const int items256 = pairs * (p.CoutPad / 256), items128 = pairs * (p.CoutPad / 128);
-    const double t256 = (double)((items256 + slots - 1) / slots), t128 = 0.6 * (double)((items128 + slots - 1) / slots);
-    if (t128 < 0.95 * t256) bn = 128;
-  }
   return bn;
 }
 
@@ -745,6 +546,8 @@ int launch_conv_tc(const ConvTcParams& p, const void* x_hi, const void* x_lo, co
     return -1;
   };
   if (p.Cin % 32) return fail("Cin must be a multiple of 32");
+  // the epilogue handles channel pairs of 8-channel groups, and its statistics shuffles need the whole warp
+  if (p.Cout % 8) return fail("Cout must be a multiple of 8");
   const bool f16 = p.f16 != 0;
   const int eb = f16 ? 2 : 4;
   // a 128-byte row holds 32 tf32 / 64 fp16 channels; 32-channel fp16 layers use the 64-byte (SWIZZLE_64B) rows
@@ -755,12 +558,11 @@ int launch_conv_tc(const ConvTcParams& p, const void* x_hi, const void* x_lo, co
   const int BN = p.force_bn ? p.force_bn : (p.fin_out ? 128 : pick_bn_for_launch(p, num_sms));
   if (variant && !p.mtn) *variant = BN;
   // 2-CTA clusters when there are at least two pixel tiles per SM pair to go around
-  const int CL = (p.cluster == 2 && (p.Mtot + BM - 1) / BM >= 2) ? 2 : 1;
+  const int CL = (p.cluster == 2 && (p.Mtot + 127) / 128 >= 2) ? 2 : 1;
   if (p.tail && !p.mtn && CL == 2 && BN == 256 && p.CoutPad == 256 && p.splits == 1) {
-    // Wave quantisation: e.g. 208 pixel tiles = 104 pairs on 74 pair slots run as two rounds, the second 40 % full.
-    // The whole rounds keep the 256-channel tile; the remaining pairs are run with 128-channel tiles (twice as many
-    // work items of ~0.6x the duration) when those fit in one round: 2.0 -> 1.6 rounds.
-    const int m_tiles = (p.Mtot + BM - 1) / BM, pairs = (m_tiles + 1) / 2, slots = p.tail > 1 ? p.tail : num_sms / 2;
+    // Wave quantisation: a 256-channel launch whose last round is partly empty runs its whole rounds with the 256-channel
+    // tile and the remaining pixel blocks with 128-channel tiles, when those fit in one round.
+    const int m_tiles = (p.Mtot + 127) / 128, pairs = (m_tiles + 1) / 2, slots = p.tail > 1 ? p.tail : num_sms / 2;
     const int full = pairs / slots, rem = pairs - full * slots;
     if (full >= 1 && rem > 0 && 2 * rem <= slots) {
       ConvTcParams q1 = p, q2 = p;
@@ -773,7 +575,8 @@ int launch_conv_tc(const ConvTcParams& p, const void* x_hi, const void* x_lo, co
   }
   ConvTcParams q = p;
   {  // split-K factor: minimise rounds(S) / S over the persistent grid (2 % penalty per extra split for the hand-over)
-    const int m_tiles = p.mtn ? p.mtn : (p.Mtot + BM - 1) / BM;
+    const int BMT = BN == 256 ? Geo<256>::BMT : Geo<128>::BMT;
+    const int m_tiles = p.mtn ? p.mtn * (128 / BMT) : (p.Mtot + BMT - 1) / BMT;
     const int tiles = ((m_tiles + CL - 1) / CL) * CL * (p.CoutPad / BN);
     // k-blocks of KBY bytes and the chunks the kernel sums them in (p.kc counts 128-byte k-blocks)
     const int nk = p.taps * (p.Cin / (KBY / eb)), kcs = p.kc * (128 / KBY);
@@ -799,12 +602,13 @@ int launch_conv_tc(const ConvTcParams& p, const void* x_hi, const void* x_lo, co
     rs = true;
     for (int t = 0; t < p.taps; ++t) {
       const int sh = p.tap_off[t] - p.tap_off[(t / ntx) * ntx];
-      if (sh < 0 || sh > CfgRS<64, 1>::AR - BM) rs = false;
+      if (sh < 0 || sh > RS_SLACK) rs = false;
     }
     q.rs_ntx = ntx, q.rs_base_offset = p.rowshare == 2 ? 1 : 0;
   }
   CUtensorMap mXh, mXl, mWh, mWl;
-  const int abox = rs ? CfgRS<64, 1>::AR : BM;
+  const int bmt = BN == 256 ? Geo<256>::BMT : Geo<128>::BMT;
+  const int abox = rs ? bmt + RS_SLACK : bmt;
   if (encode_tmap_2d(&mXh, x_hi, (uint64_t)p.Mtot, p.Cin, abox, KBY / eb, eb, KBY) ||
       encode_tmap_2d(&mXl, x_lo, (uint64_t)p.Mtot, p.Cin, abox, KBY / eb, eb, KBY) ||
       encode_tmap_2d(&mWh, w_hi, (uint64_t)p.taps * p.CoutPad, p.Cin, BN / CL, KBY / eb, eb, KBY) ||

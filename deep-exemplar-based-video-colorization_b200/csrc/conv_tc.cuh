@@ -1,4 +1,4 @@
-// tcgen05 (5th-gen tensor core) convolution engine; see conv_tc.cu.
+// Hopper tensor-core (wgmma) convolution engine; see conv_tc.cu.
 #pragma once
 #include <string>
 
@@ -32,17 +32,17 @@ struct ConvTcParams {
   const float* fin_w;
   const float* fin_b;
   float* fin_out;
-  int mt0, mtn;   // pixel-tile range [mt0, mt0 + mtn) of this launch (mtn = 0: all tiles)
+  int mt0, mtn;   // range [mt0, mt0 + mtn) of 128-pixel blocks of this launch (mtn = 0: all pixels)
   int force_bn;   // channel tile of this launch (0: chosen by the launcher)
   int tail;       // 1: a two-round 256-channel launch runs its last partial round with 128-channel tiles (see launcher);
-                  // > 1 (tests): same, pretending the GPU has `tail` pair slots
+                  // > 1 (tests): same, pretending the GPU has `tail` cluster slots
   int splits;     // split-K factor S (1 = off); needs ws / flags below
   float* ws;      // [tiles][BN][128] fp32 partial totals
   int* flags;     // [tiles], value epoch*16 + (splits completed)
   int epoch;      // unique per launch sharing `flags`
   int kbytes;     // bytes of K per pipeline stage: 64 (SWIZZLE_64B, twice the stages) or 128 (SWIZZLE_128B)
   int cluster;    // 2: run as 2-CTA clusters with TMA-multicast weight tiles; 1: single CTAs
-  int kc;         // k-blocks (32 input channels each) summed in TMEM before promotion to fp32 registers
+  int kc;         // 128-byte k-blocks summed in the wgmma accumulators before promotion to the fp32 register totals
   int rowshare;   // 1 / 2: the taps of one kernel row share one activation tile in shared memory (conv_tc.cu: CfgRS); 2 also
                   // sets the descriptors' base-offset field to the row shift; 0: one activation tile per tap
   int rs_ntx, rs_base_offset;  // filled by the launcher

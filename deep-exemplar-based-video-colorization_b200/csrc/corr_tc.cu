@@ -1,28 +1,25 @@
-// K7 on the 5th-generation tensor cores (tcgen05 + TMEM + TMA), sm_100a only.
+// K7 on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 //   f = theta_hat^T phi_hat  ->  sim = rowmax f  ->  P = softmax_j(f / T)  ->  y = P V      (NonlocalNet.py:477-498)
 //
 // fp32-class accuracy from low-precision MMAs by operand splitting: x = hi + lo with hi, lo exactly
 // representable in the MMA input type (tf32: 2 x 11 significant bits; bf16: 2 x 8), and
 //   f ~= hi_a.hi_b + hi_a.lo_b + lo_a.hi_b           (lo.lo dropped: 2^-22 resp. 2^-16 relative)
-// all three accumulated into the same fp32 TMEM tile.  A third format, FP16X3, splits x * 2^14 into two fp16 planes
+// all three accumulated into the same fp32 register tile.  A third format, FP16X3, splits x * 2^14 into two fp16 planes
 // (theta_hat / phi_hat are unit vectors, so the fixed power-of-two scale is exact and cannot overflow): the same
 // 2 x 11 significant bits as tf32 at twice the MMA rate and half the operand bytes; scores come out times 2^28.
-// FP16X3 is the default (|df| ~ 5e-7, argmax identical to fp64 on every test); DVC_MATH_TF32X3 (|df| ~ 1e-7) and
-// DVC_MATH_BF16X3 (|df| ~ 2e-6) are selectable.  By default two CTAs on adjacent query tiles run as a pair
-// (tcgen05.mma.cta_group::2, each staging half of the reference tile; Cfg<2> below); the single-CTA form:
+// FP16X3 is the default; DVC_MATH_TF32X3 and DVC_MATH_BF16X3 are selectable.  By default two CTAs on adjacent query
+// tiles run as a 2-CTA cluster that shares the reference tile: each CTA loads half of it and multicasts it to both.
 //
-// Kernel structure (one CTA = 128 query rows x a range of 256-column tiles of reference positions):
-//   warp 0      TMA producer: per k-block (128 bytes of K) loads A_hi, A_lo [128 x 128B] and B_hi, B_lo [256 x 128B]
-//               with SWIZZLE_128B into a 2-stage shared-memory ring (96 KB per stage), mbarrier expect_tx.
-//   warp 1      TMEM owner + MMA issuer: one elected thread issues 4 k-steps x 3 tcgen05.mma (M128 x N256) per
-//               stage into one of two 256-column fp32 accumulators (all 512 TMEM columns), tcgen05.commit
-//               releases the smem stage and, after the last k-block, publishes the score tile.
-//   warps 2..5  epilogue: thread t owns query row t (TMEM lane t): tcgen05.ld 32 columns at a time, running
-//               (max, argmax) or online softmax (max, sum, 3 colour sums) entirely in registers -- no
-//               cross-thread reduction; overlaps the MMAs of the next tile through the double-buffered TMEM.
-// The N x N score matrix never leaves the SM.  Column-range splits (grid.z) balance the 148 SMs; a small merge
-// kernel combines the per-split row statistics.
+// Kernel structure (one CTA = 128 query rows x a range of 256-column tiles of reference positions), 384 threads:
+//   warp 0        TMA producer: per k-block (128 bytes of K) loads A_hi, A_lo [128 x 128B] and B_hi, B_lo [256 x 128B]
+//                 with SWIZZLE_128B into a 2-stage shared-memory ring (96 KB per stage), mbarrier expect_tx.
+//   warps 4..11   two consumer warpgroups, one per 64 query rows: 4 k-steps x 3 wgmma (M64 x N256) per stage into
+//                 128 fp32 registers per thread, then the epilogue on those registers: every thread owns two query
+//                 rows and 64 of the tile's columns and keeps running (max, argmax) or online-softmax (max, sum, 3
+//                 colour sums) statistics per row; the four threads that share a row write four partial results.
+// The N x N score matrix never leaves the SM.  Column-range splits (grid.z) balance the SMs; a small merge kernel
+// combines the per-split, per-thread row statistics.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -63,44 +60,20 @@ int encode_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t c
 
 namespace {
 
-constexpr int BM = 128;        // query rows per CTA (= TMEM lanes)
-constexpr int BN = 256;        // reference positions per score tile (= TMEM columns per accumulator)
-// CL = 2: CTA pairs (tcgen05.mma.cta_group::2) on two adjacent 128-row query tiles.  The three MMAs per k-step
-// re-read both operands from shared memory, which binds a single CTA to the 128 B/clk shared-memory port (96 KB of TMA
-// writes + 144 KB of MMA reads per 1536 tensor cycles = 156 B/clk; ncu: tensor pipe 74-82 %).  In a pair each CTA
-// stages its own query rows and HALF of the reference-position tile (104 B/clk), and three 64 KB stages fit.
-template <int CL>
+constexpr int BM = 128;        // query rows per CTA (two consumer warpgroups of 64)
+constexpr int BN = 256;        // reference positions per score tile (= wgmma N)
+constexpr int NTHREADS = 384;  // warpgroup 0: TMA producer (warp 0); warpgroups 1, 2: MMA + epilogue
+constexpr int CONSUMER_WARPS = 8;
+constexpr int QUADS = 4;       // threads sharing a query row (wgmma accumulator layout): partial results per row and split
+// Each CTA holds the whole reference tile of a stage (in a 2-CTA cluster half of it arrives by the peer's multicast).
 struct Cfg {
-  static constexpr int STAGES = CL == 2 ? 3 : 2;
-  static constexpr int A_BYTES = BM * 128, B_BYTES = (BN / CL) * 128;
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;  // 98304 / 65536
+  static constexpr int STAGES = 2;
+  static constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128;
+  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;  // 98304
   static constexpr int V_RING_BYTES = 2 * BN * 16;  // softmax epilogue: the V rows of the tile in flight, two slots
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/ + V_RING_BYTES;
 };
-// warp 0 TMA, warp 1 MMA, then 8 epilogue warps: two per TMEM lane quarter, each owning 128 of the tile's 256 columns --
-// twice the threads to hide the tcgen05.ld / exp2 / FMA latency chains behind (with 4 warps the exact argmax kernel ran at
-// 39 % tensor-pipe activity under ncu, the 8-warp softmax kernel at 71 %)
-template <bool SOFTMAX>
-struct Epi {
-  static constexpr int WARPS = 8;
-  static constexpr int HALVES = WARPS / 4;
-  static constexpr int NTHREADS = 64 + 32 * WARPS;
-};
 
-// packed fp32 pair arithmetic (Blackwell FFMA2): acc.{x,y} += a.{x,y} * b.{x,y}
-__device__ __forceinline__ void fma2(unsigned long long& acc, unsigned long long a, unsigned long long b) {
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b));
-}
-__device__ __forceinline__ unsigned long long pack2(float x, float y) {
-  unsigned long long r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(x), "f"(y));
-  return r;
-}
-__device__ __forceinline__ float2 unpack2(unsigned long long v) {
-  float2 r;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v));
-  return r;
-}
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -111,6 +84,20 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(tc::smem_u32(smem_dst)),
                "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(tc::smem_u32(bar))
                : "memory");
+}
+// a consumer warp hands a ring stage back: in a cluster the stage of EVERY CTA must be free before a producer
+// multicasts into it, so each consumer warp arrives on the "empty" barrier of both CTAs
+template <int CL>
+__device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
+  __syncwarp();
+  if (lane == 0) {
+    if (CL == 1) {
+      tc::mbar_arrive(bar);
+    } else {
+#pragma unroll
+      for (int r = 0; r < CL; ++r) tc::mbar_arrive_cluster(bar, (uint32_t)r);
+    }
+  }
 }
 
 // per (split part, row) partial statistics.  Softmax: running max m, sum s of exp weights, weighted colour sums a*.
@@ -128,9 +115,9 @@ struct TcParams {
   int tiles_per_split;
   float sc;  // log2(e) / T
   const float* row_sc;  // optional per-query-row log2(e) / T_i (overrides sc): the contextual loss normalises every row by its own minimum distance
-  float out_scale;  // scores in TMEM are true scores / out_scale (2^-28 for pre-scaled fp16 operands, else 1)
+  float out_scale;  // scores in the accumulators are true scores / out_scale (2^-28 for pre-scaled fp16 operands, else 1)
   const float4* V;
-  SplitOut* part;  // [nsplit][B*NA]
+  SplitOut* part;  // [nsplit * QUADS][B*NA]
 };
 
 // ---- operand split: rows [R][C] fp32 -> hi / lo planes -----------------------------------------------
@@ -224,29 +211,21 @@ __global__ void __launch_bounds__(256) screen_planes_kernel(const float* __restr
 
 // ---- main kernel ---------------------------------------------------------------------------------------
 template <int FMT, bool SOFTMAX, int CL>
-__global__ void __launch_bounds__(Epi<SOFTMAX>::NTHREADS, 1)
+__global__ void __launch_bounds__(NTHREADS, 1)
     corr_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                    const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, const TcParams p) {
-  constexpr bool TF32 = (FMT == 0);
-  constexpr int KB = TF32 ? 32 : 64;       // K elements per 128-byte k-block
-  constexpr int UMMA_K_BYTES = 32;         // one MMA consumes 32 bytes of K (8 tf32 / 16 bf16)
-  constexpr uint32_t IDESC = tc::umma_idesc(FMT == 0 ? 2u : (FMT == 1 ? 1u : 0u), BM * CL, BN);  // tf32 / bf16 / f16
-  constexpr int STAGES = Cfg<CL>::STAGES, A_BYTES = Cfg<CL>::A_BYTES, B_BYTES = Cfg<CL>::B_BYTES;
-  constexpr int STAGE_BYTES = Cfg<CL>::STAGE_BYTES;
+  constexpr int KB = FMT == 0 ? 32 : 64;   // K elements per 128-byte k-block
+  constexpr int STAGES = Cfg::STAGES, A_BYTES = Cfg::A_BYTES, B_BYTES = Cfg::B_BYTES, STAGE_BYTES = Cfg::STAGE_BYTES;
   const int crank = (CL == 2) ? (int)tc::cluster_ctarank() : 0;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* full = bars;                 // [STAGES]   TMA -> MMA
-  uint64_t* empty = bars + STAGES;       // [STAGES]   MMA -> TMA
-  uint64_t* tfull = bars + 2 * STAGES;   // [2]        MMA -> epilogue
-  uint64_t* tempty = bars + 2 * STAGES + 2;  // [2]    epilogue -> MMA
-  uint64_t* vfull = bars + 2 * STAGES + 4;   // [2]    bulk copy of the tile's V rows -> epilogue (softmax)
-  uint64_t* vempty = bars + 2 * STAGES + 6;  // [2]    this CTA's epilogue -> its producer (softmax)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 8);
+  uint64_t* full = bars;                     // [STAGES]   TMA -> MMA
+  uint64_t* empty = bars + STAGES;           // [STAGES]   MMA (both CTAs of a cluster) -> TMA
+  uint64_t* vfull = bars + 2 * STAGES;       // [2]        bulk copy of the tile's V rows -> epilogue (softmax)
+  uint64_t* vempty = bars + 2 * STAGES + 2;  // [2]        this CTA's epilogue -> its producer (softmax)
   float4* v_ring = reinterpret_cast<float4*>(smem + STAGES * STAGE_BYTES + 256);  // [2][BN]
-  constexpr int EPI_WARPS = Epi<SOFTMAX>::WARPS;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.y;
@@ -263,32 +242,17 @@ __global__ void __launch_bounds__(Epi<SOFTMAX>::NTHREADS, 1)
     tc::tma_prefetch_desc(&tmAl);
     tc::tma_prefetch_desc(&tmBh);
     tc::tma_prefetch_desc(&tmBl);
-    for (int i = 0; i < STAGES; ++i) tc::mbar_init(&full[i], 1), tc::mbar_init(&empty[i], 1);
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&tfull[i], 1), tc::mbar_init(&tempty[i], EPI_WARPS * CL);  // pair: both epilogues
-      tc::mbar_init(&vfull[i], 1), tc::mbar_init(&vempty[i], EPI_WARPS);
-    }
+    for (int i = 0; i < STAGES; ++i) tc::mbar_init(&full[i], 1), tc::mbar_init(&empty[i], CONSUMER_WARPS * CL);
+    for (int i = 0; i < 2; ++i) tc::mbar_init(&vfull[i], 1), tc::mbar_init(&vempty[i], CONSUMER_WARPS);
     tc::fence_barrier_init();
   }
-  if (CL == 2) tc::cluster_sync_all();  // both CTAs are resident before the pair allocation
-  if (warp == 1) {
-    if (CL == 2) {
-      tc::tmem_alloc_pair(tmem_slot, 512);
-      tc::tmem_relinquish_pair();
-    } else {
-      tc::tmem_alloc(tmem_slot, 512);
-      tc::tmem_relinquish();
-    }
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  if (CL == 2) tc::cluster_sync_all();  // the peer's barriers are initialised before any remote arrive reaches them
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (CL == 2) tc::cluster_sync_all();  // the peer's barriers are initialised before any multicast or remote arrive reaches them
 
-  if (warp == 0) {
-    // ================= TMA producer (warp-convergent loop, one elected lane issues) =================
-    {
+  if (warp < 4) {
+    tc::setmaxnreg_dec<40>();
+    if (warp == 0) {
+      // ================= TMA producer (warp-convergent loop, one elected lane issues) =================
       int stage = 0;
       uint32_t phase = 0;
       for (int t = 0; t < ntiles; ++t) {
@@ -297,28 +261,23 @@ __global__ void __launch_bounds__(Epi<SOFTMAX>::NTHREADS, 1)
           tc::mbar_wait(&empty[stage], phase ^ 1);
           if (tc::elect_one()) {
             uint8_t* st = smem + stage * STAGE_BYTES;
+            tc::mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
+            tc::tma_load_2d(st, &tmAh, &full[stage], kb * KB, b * p.NA + m0);
+            tc::tma_load_2d(st + A_BYTES, &tmAl, &full[stage], kb * KB, b * p.NA + m0);
             if (CL == 1) {
-              tc::mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
-              tc::tma_load_2d(st, &tmAh, &full[stage], kb * KB, b * p.NA + m0);
-              tc::tma_load_2d(st + A_BYTES, &tmAl, &full[stage], kb * KB, b * p.NA + m0);
               tc::tma_load_2d(st + 2 * A_BYTES, &tmBh, &full[stage], kb * KB, col0);
               tc::tma_load_2d(st + 2 * A_BYTES + B_BYTES, &tmBl, &full[stage], kb * KB, col0);
-            } else {  // my query rows and my half of the reference positions; the leader's barrier counts all bytes
-              if (crank == 0) tc::mbar_arrive_expect_tx(&full[stage], 2 * STAGE_BYTES);
-              const int hrow = crank * (BN / 2);
-              tc::tma_load_2d_pair(st, &tmAh, &full[stage], kb * KB, b * p.NA + m0);
-              tc::tma_load_2d_pair(st + A_BYTES, &tmAl, &full[stage], kb * KB, b * p.NA + m0);
-              tc::tma_load_2d_pair(st + 2 * A_BYTES, &tmBh, &full[stage], kb * KB, col0 + hrow);
-              tc::tma_load_2d_pair(st + 2 * A_BYTES + B_BYTES, &tmBl, &full[stage], kb * KB, col0 + hrow);
+            } else {  // my half of the reference positions, multicast into both CTAs of the cluster
+              const int h = crank * (BN / 2);
+              tc::tma_load_2d_mc(st + 2 * A_BYTES + h * 128, &tmBh, &full[stage], kb * KB, col0 + h, 3);
+              tc::tma_load_2d_mc(st + 2 * A_BYTES + B_BYTES + h * 128, &tmBl, &full[stage], kb * KB, col0 + h, 3);
             }
           }
           __syncwarp();
           if (++stage == STAGES) stage = 0, phase ^= 1;
         }
         if (SOFTMAX) {
-          // the V rows of this tile's columns for my own epilogue.  Issued after the tile's last k-block: by then the
-          // MMAs of this tile have started, so the slot (freed together with the accumulator of tile t-2) is free and
-          // the wait below never delays the operand prefetch.
+          // the V rows of this tile's columns for this CTA's epilogue; the slot was freed by the epilogue of tile t-2
           const int buf = t & 1;
           tc::mbar_wait(&vempty[buf], ((t >> 1) & 1) ^ 1);
           if (tc::elect_one()) {
@@ -331,204 +290,148 @@ __global__ void __launch_bounds__(Epi<SOFTMAX>::NTHREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer (warp-convergent loop, one elected lane issues; pair: leader CTA only) =====
-    if (CL == 1 || crank == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = 0; t < ntiles; ++t) {
-        const int buf = t & 1;
-        const uint32_t acc_phase = (t >> 1) & 1;
-        tc::mbar_wait(&tempty[buf], acc_phase ^ 1);
-        tc::tc_fence_after();
-        const uint32_t d = tmem_base + buf * BN;
-        for (int kb = 0; kb < nkb; ++kb) {
-          tc::mbar_wait(&full[stage], phase);
-          tc::tc_fence_after();
-          const uint32_t sa = tc::smem_u32(smem + stage * STAGE_BYTES);
-          const uint64_t dAh = tc::umma_desc_k128(sa), dAl = tc::umma_desc_k128(sa + A_BYTES);
-          const uint64_t dBh = tc::umma_desc_k128(sa + 2 * A_BYTES), dBl = tc::umma_desc_k128(sa + 2 * A_BYTES + B_BYTES);
-          if (tc::elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < 128 / UMMA_K_BYTES; ++kk) {
-              const uint64_t adv = (uint64_t)((kk * UMMA_K_BYTES) >> 4);  // start-address field is in 16-byte units
-              // small cross terms first, the dominant hi.hi term last
-              if (CL == 1) {
-                tc::umma_ss<TF32>(d, dAl + adv, dBh + adv, IDESC, (kb | kk) ? 1u : 0u);
-                tc::umma_ss<TF32>(d, dAh + adv, dBl + adv, IDESC, 1u);
-                tc::umma_ss<TF32>(d, dAh + adv, dBh + adv, IDESC, 1u);
-              } else {
-                tc::umma_ss_pair<TF32>(d, dAl + adv, dBh + adv, IDESC, (kb | kk) ? 1u : 0u);
-                tc::umma_ss_pair<TF32>(d, dAh + adv, dBl + adv, IDESC, 1u);
-                tc::umma_ss_pair<TF32>(d, dAh + adv, dBh + adv, IDESC, 1u);
-              }
-            }
-            if (CL == 1) {
-              tc::umma_commit(&empty[stage]);  // smem stage reusable once these MMAs have read it
-              if (kb == nkb - 1) tc::umma_commit(&tfull[buf]);
-            } else {
-              tc::umma_commit_pair_mc(&empty[stage], 3);
-              if (kb == nkb - 1) tc::umma_commit_pair_mc(&tfull[buf], 3);
-            }
-          }
-          __syncwarp();
-          if (++stage == STAGES) stage = 0, phase ^= 1;
-        }
-      }
-    }
   } else {
-    // ================= epilogue: one query row per thread (softmax: per thread and column half) =================
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;  // which 128 columns of every 256-column tile
-    constexpr int COLS = BN / Epi<SOFTMAX>::HALVES;     // columns per thread and tile
-    const int row_local = q * 32 + lane;
-    const int row = m0 + row_local;
-    // exponent scale in units of the (possibly pre-scaled) TMEM scores
-    const float sck = (p.row_sc ? __ldg(p.row_sc + (size_t)b * p.NA + min(m0 + q * 32 + lane, p.NA - 1)) : p.sc) * p.out_scale;
-    float run_m = -INFINITY;
-    // argmax: number of bit-equal maxima and the sum of their V rows; softmax: (a0, a1) and (a2, s) as packed pairs
-    float cnt = 0.f, t0s = 0.f, t1s = 0.f, t2s = 0.f;
-    unsigned long long acc01 = 0ull, acc2s = 0ull;
-    int run_i = 0;
+    // ================= consumers: wgmma into registers, then the epilogue on them =================
+    tc::setmaxnreg_inc<232>();
+    const int wg = (warp >> 2) - 1, qd = lane & 3;
+    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // local query row of slot 0 (slot 1: rl + 8)
+    const uint32_t a_off = (uint32_t)(wg * 64 * 128);
+    float sck[2], run_m[2] = {-INFINITY, -INFINITY};
+    // argmax: number of bit-equal maxima and the sum of their V rows; softmax: weighted colour sums and the sum of weights
+    float cnt[2] = {0.f, 0.f}, s0[2] = {0.f, 0.f}, s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
+    int run_i[2] = {0, 0};
+#pragma unroll
+    for (int h = 0; h < 2; ++h)  // exponent scale in units of the (possibly pre-scaled) accumulator scores
+      sck[h] = (p.row_sc ? __ldg(p.row_sc + (size_t)b * p.NA + min(m0 + rl + 8 * h, p.NA - 1)) : p.sc) * p.out_scale;
     const float4* __restrict__ Vg = p.V + (size_t)bphi * p.NB;
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
     for (int t = 0; t < ntiles; ++t) {
-      const int buf = t & 1;
-      const uint32_t acc_phase = (t >> 1) & 1;
-      tc::mbar_wait(&tfull[buf], acc_phase);
-      if (SOFTMAX) tc::mbar_wait(&vfull[buf], acc_phase);
-      tc::tc_fence_after();
-      const int colbase = (t0 + t) * BN + half * COLS;
-      const float4* Vs = v_ring + buf * BN + half * COLS;
-#pragma unroll 1
-      for (int c0 = 0; c0 < COLS / 32; c0 += 2) {
-        if (colbase + c0 * 32 >= p.NB) break;  // warp-uniform
-        // two loads in flight per wait: a tcgen05.ld that is waited for alone exposes its whole latency
-        uint32_t r2[2][32];
-        __syncwarp();  // tcgen05.ld is .sync.aligned: the warp must be converged
-        tc::tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN + half * COLS + c0 * 32, r2[0]);
-        tc::tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN + half * COLS + c0 * 32 + 32, r2[1]);
-        tc::tmem_ld_wait();
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        tc::mbar_wait(&full[stage], phase);
+        const uint32_t sa = tc::smem_u32(smem + stage * STAGE_BYTES);
+        const uint64_t dAh = tc::wg_desc_k128(sa + a_off), dAl = tc::wg_desc_k128(sa + A_BYTES + a_off);
+        const uint64_t dBh = tc::wg_desc_k128(sa + 2 * A_BYTES), dBl = tc::wg_desc_k128(sa + 2 * A_BYTES + B_BYTES);
+        tc::wg_fence_regs(acc);
+        tc::wg_fence();
 #pragma unroll
-      for (int cj = 0; cj < 2; ++cj) {
-        const int c = c0 + cj;
-        const int cb = colbase + c * 32;
-        if (cb >= p.NB) continue;  // warp-uniform
-        uint32_t (&r)[32] = r2[cj];
-        const int nvalid = min(32, p.NB - cb);
-        float cm = -INFINITY;
-        if (nvalid == 32) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) cm = fmaxf(cm, __uint_as_float(r[i]));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (i < nvalid) cm = fmaxf(cm, __uint_as_float(r[i]));
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint64_t adv = (uint64_t)(kk * 2);  // 32 bytes of K, in 16-byte units of the start-address field
+          // small cross terms first, the dominant hi.hi term last
+          tc::wgmma_fmt<FMT>(acc, dAl + adv, dBh + adv, (kb | kk) ? 1u : 0u);
+          tc::wgmma_fmt<FMT>(acc, dAh + adv, dBl + adv, 1u);
+          tc::wgmma_fmt<FMT>(acc, dAh + adv, dBh + adv, 1u);
         }
-        if (!SOFTMAX) {
-          if (cm >= run_m) {  // rare once the running maximum has settled
-            if (cm > run_m) run_m = cm, cnt = 0.f, t0s = t1s = t2s = 0.f;
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (i < nvalid && __uint_as_float(r[i]) == cm) {
-                if (cnt == 0.f) run_i = cb + i;  // lowest index attaining the maximum
-                const float4 v = __ldg(Vg + cb + i);
-                cnt += 1.f, t0s += v.x, t1s += v.y, t2s += v.z;
-              }
-          }
-        } else {
-          if (cm > run_m) {
-            const float sc_old = (run_m == -INFINITY) ? 0.f : ex2_approx((run_m - cm) * sck);
-            const unsigned long long sc2 = pack2(sc_old, sc_old);
-            unsigned long long z = 0ull;
-            fma2(z, acc01, sc2), acc01 = z, z = 0ull;
-            fma2(z, acc2s, sc2), acc2s = z;
-            run_m = cm;
-          }
-          // weights e = 2^((f - m) * log2(e) / T); V rows come from shared memory as (L, a | b, 1): two packed FMAs
-          // accumulate (a0, a1) and (a2, sum of weights)
-          if (nvalid == 32) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const float e = ex2_approx((__uint_as_float(r[i]) - run_m) * sck);
-              const ulonglong2 vv = *reinterpret_cast<const ulonglong2*>(Vs + c * 32 + i);
-              const unsigned long long e2 = pack2(e, e);
-              fma2(acc01, e2, vv.x), fma2(acc2s, e2, vv.y);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (i < nvalid) {
-                const float e = ex2_approx((__uint_as_float(r[i]) - run_m) * sck);
-                const ulonglong2 vv = *reinterpret_cast<const ulonglong2*>(Vs + c * 32 + i);
-                const unsigned long long e2 = pack2(e, e);
-                fma2(acc01, e2, vv.x), fma2(acc2s, e2, vv.y);
-              }
-          }
+        tc::wg_commit();
+        if (prev >= 0) {  // the previous k-block's MMAs have read their stage: hand it back
+          tc::wg_wait<1>();
+          release_stage<CL>(&empty[prev], lane);
         }
-      }  // cj
+        prev = stage;
+        if (++stage == STAGES) stage = 0, phase ^= 1;
       }
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CL == 1)
-          tc::mbar_arrive(&tempty[buf]);
-        else
-          tc::mbar_arrive_leader(&tempty[buf]);
-        if (SOFTMAX) tc::mbar_arrive(&vempty[buf]);
+      tc::wg_wait<0>();
+      tc::wg_fence_regs(acc);
+      release_stage<CL>(&empty[prev], lane);
+
+      const int buf = t & 1;
+      if (SOFTMAX) tc::mbar_wait(&vfull[buf], (t >> 1) & 1);
+      const int colbase = (t0 + t) * BN;
+      const bool full_tile = colbase + BN <= p.NB;
+      const float4* Vs = v_ring + buf * BN;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        // this thread's columns of the tile: 8 j + 2 qd + e, j = 0..31, e = 0, 1 (ascending)
+        float cm = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (full_tile || colbase + 8 * j + 2 * qd + e < p.NB) cm = fmaxf(cm, acc[4 * j + 2 * h + e]);
+        if (!SOFTMAX) {
+          if (cm >= run_m[h]) {  // rare once the running maximum has settled
+            if (cm > run_m[h]) run_m[h] = cm, cnt[h] = 0.f, s0[h] = s1[h] = s2[h] = 0.f;
+            uint64_t hit = 0;  // bit 2 j + e: column 8 j + 2 qd + e attains the maximum
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                hit |= (uint64_t)(acc[4 * j + 2 * h + e] == cm && (full_tile || colbase + 8 * j + 2 * qd + e < p.NB)) << (2 * j + e);
+            while (hit) {  // ascending columns
+              const int i = __ffsll((long long)hit) - 1;
+              hit &= hit - 1;
+              const int col = colbase + 8 * (i >> 1) + 2 * qd + (i & 1);
+              if (cnt[h] == 0.f) run_i[h] = col;  // lowest index of this thread's columns attaining the maximum
+              const float4 v = __ldg(Vg + col);
+              cnt[h] += 1.f, s0[h] += v.x, s1[h] += v.y, s2[h] += v.z;
+            }
+          }
+        } else {
+          if (cm > run_m[h]) {
+            const float sc_old = (run_m[h] == -INFINITY) ? 0.f : ex2_approx((run_m[h] - cm) * sck[h]);
+            s0[h] *= sc_old, s1[h] *= sc_old, s2[h] *= sc_old, cnt[h] *= sc_old;
+            run_m[h] = cm;
+          }
+          // weights e = 2^((f - m) * log2(e) / T); V rows come from shared memory as (a0, a1, a2, 1)
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int cl = 8 * j + 2 * qd + e;
+              if (full_tile || colbase + cl < p.NB) {
+                const float w = ex2_approx((acc[4 * j + 2 * h + e] - run_m[h]) * sck[h]);
+                const float4 v = Vs[cl];
+                s0[h] = fmaf(w, v.x, s0[h]), s1[h] = fmaf(w, v.y, s1[h]), s2[h] = fmaf(w, v.z, s2[h]), cnt[h] = fmaf(w, v.w, cnt[h]);
+              }
+            }
+        }
+      }
+      if (SOFTMAX) {
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&vempty[buf]);
       }
     }
-    if (row < p.NA) {
-      SplitOut o;
-      o.m = run_m * p.out_scale, o.idx = run_i, o.pad0 = o.pad1 = 0.f;
-      if (SOFTMAX) {
-        const float2 x01 = unpack2(acc01), x2s = unpack2(acc2s);
-        o.s = x2s.y, o.a0 = x01.x, o.a1 = x01.y, o.a2 = x2s.x;
-      } else {
-        o.s = cnt, o.a0 = t0s, o.a1 = t1s, o.a2 = t2s;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = m0 + rl + 8 * h;
+      if (row < p.NA) {
+        SplitOut o;
+        o.m = run_m[h] * p.out_scale, o.idx = run_i[h], o.pad0 = o.pad1 = 0.f;
+        o.s = cnt[h], o.a0 = s0[h], o.a1 = s1[h], o.a2 = s2[h];
+        p.part[((size_t)(blockIdx.z * QUADS + qd) * p.B + b) * p.NA + row] = o;
       }
-      p.part[((size_t)(blockIdx.z * Epi<SOFTMAX>::HALVES + half) * p.B + b) * p.NA + row] = o;
     }
   }
 
-  tc::tc_fence_before();
   __syncthreads();
-  if (CL == 2) tc::cluster_sync_all();  // the leader's MMAs read the peer's shared memory until the very end
-  if (warp == 1) {
-    tc::tc_fence_after();
-    if (CL == 2)
-      tc::tmem_dealloc_pair(tmem_base, 512);
-    else
-      tc::tmem_dealloc(tmem_base, 512);
-  }
+  if (CL == 2) tc::cluster_sync_all();  // no CTA may exit while its peer can still multicast into it or arrive on its barriers
 }
+
 
 // ---- screened T -> 0 path: one fp16 pass + exact re-scoring of the candidates ----------------------------------------
 // At T <= 2e-10 only the row maximum matters (one-hot softmax), and a single hi.hi pass locates it up to the
 // rigorous error eps_i of row i (screen_planes_kernel): every column j with f_screen(i, j) >= max_j f_screen - 2 eps_i is a
 // CANDIDATE, all others are provably not the maximum.  The screening kernel keeps up to SCREEN_K candidates per (row,
-// column-range split) while it streams the tiles -- one third of the MMA work and half of the operand bytes of the
-// 3-pass kernel; corr_rescore_kernel then evaluates the candidates exactly in fp32 on the CUDA cores (a few per row) and
-// produces (sim, argmax, mean V of bit-equal maxima).  A list that overflows marks its (row, split) for brute force.
-constexpr int SCREEN_K = 16;        // candidates kept per (row, column-range split, column half)
-constexpr int SCREEN_EPI_WARPS = 8;  // two per TMEM lane quarter, each owning 128 of a tile's 256 columns
-constexpr int SCREEN_HALVES = SCREEN_EPI_WARPS / 4;
+// column-range split, thread of the row's quad) while it streams the tiles -- one third of the MMA work and half of the
+// operand bytes of the 3-pass kernel; corr_rescore_kernel then evaluates the candidates exactly in fp32 on the CUDA cores
+// (a few per row) and produces (sim, argmax, mean V of bit-equal maxima).  A list that overflows marks its part for brute force.
+constexpr int SCREEN_K = 16;  // candidates kept per (row, column-range split, quad thread)
 
 // The query tile (128 rows x 256 channels of fp16 = 64 KB) stays RESIDENT in shared memory for the CTA's whole sweep over
-// the reference positions; only the reference tiles stream through the ring.  The kernel is bound by the L2 -> SM fabric
-// (ncu: l1tex__m_xbar2l1tex_read_bytes at 4.6 TB/s with both operands streamed; the exact 3-pass kernel pulls 6.6 TB/s, the
-// most any kernel of this library gets out of the L2), so halving the bytes per tile is what shortens it.
-template <int CL>
+// the reference positions; only the reference tiles stream through the ring: half of the bytes per tile.
 struct ScreenCfg {
-  static constexpr int STAGES = CL == 2 ? 8 : 4;
-  static constexpr int A_BYTES = BM * 128, B_BYTES = (BN / CL) * 128;
+  static constexpr int STAGES = 3;
+  static constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128;
   static constexpr int A_RES_BYTES = 4 * A_BYTES;        // all four k-blocks of the query tile (C = 256)
-  static constexpr int STAGE_BYTES = B_BYTES;            // 16384 / 32768
-  // candidate lists of the epilogue threads: [SCREEN_K][epilogue threads] column indices -- slot k of thread t lives at
-  // [k][t], so dynamic slot indices never conflict on a bank and never touch local memory
-  static constexpr int LIST_BYTES = SCREEN_K * SCREEN_EPI_WARPS * 32 * 4;
+  static constexpr int STAGE_BYTES = B_BYTES;            // 32768
+  // candidate lists of the consumer threads: [SCREEN_K][consumer threads][2 rows] column indices -- slot k of (thread, row)
+  // lives at [k][thread][row], so dynamic slot indices never conflict on a bank and never touch local memory
+  static constexpr int LT = CONSUMER_WARPS * 32 * 2;
+  static constexpr int LIST_BYTES = SCREEN_K * LT * 4;
   static constexpr int SMEM_BYTES = A_RES_BYTES + STAGES * STAGE_BYTES + 1024 + 256 + LIST_BYTES;
 };
-constexpr int SCREEN_THREADS = 64 + 32 * SCREEN_EPI_WARPS;
 
 struct ScreenParams {
   int NA, NB, B, Bphi, C;
@@ -542,17 +445,16 @@ struct ScreenParams {
   int* pidx;     // [parts][B*NA][SCREEN_K]  candidate columns
 };
 
-// 2 * eps_i in true-score units (see screen_planes_kernel); 64 * 2^-24 covers the truncating TMEM accumulation
+// 2 * eps_i in true-score units (see screen_planes_kernel); 64 * 2^-24 covers the truncating fp32 accumulation
 __device__ __forceinline__ float screen_threshold(float nd_a, float nh_a, float nd_b, float nh_b) {
   return 2.f * (nd_a * (nh_b + nd_b) + nh_a * nd_b + 4e-6f) * 1.001f;
 }
 
 template <int CL>
-__global__ void __launch_bounds__(SCREEN_THREADS, 1)
+__global__ void __launch_bounds__(NTHREADS, 1)
     corr_screen_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmBh, const ScreenParams p) {
-  using C = ScreenCfg<CL>;
+  using C = ScreenCfg;
   constexpr int KB = 64;
-  constexpr uint32_t IDESC = tc::umma_idesc(0u, BM * CL, BN);
   constexpr int STAGES = C::STAGES, A_BYTES = C::A_BYTES, STAGE_BYTES = C::STAGE_BYTES, A_RES = C::A_RES_BYTES;
   const int crank = (CL == 2) ? (int)tc::cluster_ctarank() : 0;
 
@@ -562,11 +464,8 @@ __global__ void __launch_bounds__(SCREEN_THREADS, 1)
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + STAGES * STAGE_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = bars + 2 * STAGES + 2;
-  uint64_t* afull = bars + 2 * STAGES + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 5);
-  int* s_ci = reinterpret_cast<int*>(ring + STAGES * STAGE_BYTES + 256);  // [SCREEN_K][epilogue threads] candidate columns
+  uint64_t* afull = bars + 2 * STAGES;
+  int* s_ci = reinterpret_cast<int*>(ring + STAGES * STAGE_BYTES + 256);  // [SCREEN_K][LT] candidate columns
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.y;
@@ -580,88 +479,35 @@ __global__ void __launch_bounds__(SCREEN_THREADS, 1)
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tmAh);
     tc::tma_prefetch_desc(&tmBh);
-    for (int i = 0; i < STAGES; ++i) tc::mbar_init(&full[i], 1), tc::mbar_init(&empty[i], 1);
-    for (int i = 0; i < 2; ++i) tc::mbar_init(&tfull[i], 1), tc::mbar_init(&tempty[i], SCREEN_EPI_WARPS * CL);
+    for (int i = 0; i < STAGES; ++i) tc::mbar_init(&full[i], 1), tc::mbar_init(&empty[i], CONSUMER_WARPS * CL);
     tc::mbar_init(afull, 1);
     tc::fence_barrier_init();
   }
-  if (CL == 2) tc::cluster_sync_all();
-  if (warp == 1) {
-    if (CL == 2) {
-      tc::tmem_alloc_pair(tmem_slot, 512);
-      tc::tmem_relinquish_pair();
-    } else {
-      tc::tmem_alloc(tmem_slot, 512);
-      tc::tmem_relinquish();
-    }
-  }
-  tc::tc_fence_before();
   __syncthreads();
   if (CL == 2) tc::cluster_sync_all();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    int stage = 0;
-    uint32_t phase = 0;
-    if (ntiles > 0 && tc::elect_one()) {  // the query tile: loaded once, resident for the whole sweep
-      if (CL == 1) {
-        tc::mbar_arrive_expect_tx(afull, A_RES);
-        for (int kb = 0; kb < nkb; ++kb) tc::tma_load_2d(smem + kb * A_BYTES, &tmAh, afull, kb * KB, b * p.NA + m0);
-      } else {
-        if (crank == 0) tc::mbar_arrive_expect_tx(afull, 2 * A_RES);
-        for (int kb = 0; kb < nkb; ++kb) tc::tma_load_2d_pair(smem + kb * A_BYTES, &tmAh, afull, kb * KB, b * p.NA + m0);
-      }
-    }
-    __syncwarp();
-    for (int t = 0; t < ntiles; ++t) {
-      const int col0 = bphi * p.NB + (t0 + t) * BN;
-      for (int kb = 0; kb < nkb; ++kb) {
-        tc::mbar_wait(&empty[stage], phase ^ 1);
-        if (tc::elect_one()) {
-          uint8_t* st = ring + stage * STAGE_BYTES;
-          if (CL == 1) {
-            tc::mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
-            tc::tma_load_2d(st, &tmBh, &full[stage], kb * KB, col0);
-          } else {
-            if (crank == 0) tc::mbar_arrive_expect_tx(&full[stage], 2 * STAGE_BYTES);
-            tc::tma_load_2d_pair(st, &tmBh, &full[stage], kb * KB, col0 + crank * (BN / 2));
-          }
-        }
-        __syncwarp();
-        if (++stage == STAGES) stage = 0, phase ^= 1;
-      }
-    }
-  } else if (warp == 1) {
-    if (CL == 1 || crank == 0) {
+  if (warp < 4) {
+    tc::setmaxnreg_dec<40>();
+    if (warp == 0) {
       int stage = 0;
       uint32_t phase = 0;
+      if (ntiles > 0 && tc::elect_one()) {  // the query tile: loaded once, resident for the whole sweep
+        tc::mbar_arrive_expect_tx(afull, A_RES);
+        for (int kb = 0; kb < nkb; ++kb) tc::tma_load_2d(smem + kb * A_BYTES, &tmAh, afull, kb * KB, b * p.NA + m0);
+      }
+      __syncwarp();
       for (int t = 0; t < ntiles; ++t) {
-        const int buf = t & 1;
-        if (t == 0) tc::mbar_wait(afull, 0);
-        tc::mbar_wait(&tempty[buf], ((t >> 1) & 1) ^ 1);
-        tc::tc_fence_after();
-        const uint32_t d = tmem_base + buf * BN;
+        const int col0 = bphi * p.NB + (t0 + t) * BN;
         for (int kb = 0; kb < nkb; ++kb) {
-          tc::mbar_wait(&full[stage], phase);
-          tc::tc_fence_after();
-          const uint64_t dA = tc::umma_desc_k128(tc::smem_u32(smem + kb * A_BYTES));
-          const uint64_t dB = tc::umma_desc_k128(tc::smem_u32(ring + stage * STAGE_BYTES));
+          tc::mbar_wait(&empty[stage], phase ^ 1);
           if (tc::elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              const uint64_t adv = (uint64_t)((kk * 32) >> 4);
-              if (CL == 1)
-                tc::umma_ss<false>(d, dA + adv, dB + adv, IDESC, (kb | kk) ? 1u : 0u);
-              else
-                tc::umma_ss_pair<false>(d, dA + adv, dB + adv, IDESC, (kb | kk) ? 1u : 0u);
-            }
+            uint8_t* st = ring + stage * STAGE_BYTES;
+            tc::mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
             if (CL == 1) {
-              tc::umma_commit(&empty[stage]);
-              if (kb == nkb - 1) tc::umma_commit(&tfull[buf]);
+              tc::tma_load_2d(st, &tmBh, &full[stage], kb * KB, col0);
             } else {
-              tc::umma_commit_pair_mc(&empty[stage], 3);
-              if (kb == nkb - 1) tc::umma_commit_pair_mc(&tfull[buf], 3);
+              const int h = crank * (BN / 2);
+              tc::tma_load_2d_mc(st + h * 128, &tmBh, &full[stage], kb * KB, col0 + h, 3);
             }
           }
           __syncwarp();
@@ -670,98 +516,102 @@ __global__ void __launch_bounds__(SCREEN_THREADS, 1)
       }
     }
   } else {
-    // ================= epilogue: one query row x one column half per thread =================
-    // Per tile a thread drains its 128 columns with four tcgen05.ld in flight before one wait (a load that is waited for
-    // alone exposes its full latency: the first version, one x32 load per wait, spent 7.5 K cycles per tile on a 2 K-cycle
-    // MMA tile -- as did the exact 3-pass kernel's epilogue, which hid behind its 6 K cycles of MMAs), then 16 three-input
-    // maxima per 32-column chunk.  A chunk whose maximum comes within the threshold of the row's running maximum (a
-    // "record" or a near-tie: ~ln(#chunks) times per row, but for SOME lane of a warp in about every second chunk) builds
-    // a 32-bit mask of its qualifying columns and appends their indices to the thread's list in shared memory
-    // ([slot][thread]: no bank conflicts, no local memory).  Values are not kept: a record that beats the previous maximum
-    // by more than the threshold disqualifies the whole list at once (every entry is <= the previous maximum); otherwise
-    // the old entries stay -- at worst a few extra candidates for the exact re-scoring, never a missing one.
-    const int q = warp & 3, half = (warp - 2) >> 2;
-    constexpr int COLS = BN / SCREEN_HALVES;   // 128
-    constexpr int LT = SCREEN_EPI_WARPS * 32;  // list stride
-    const int et = threadIdx.x - 64;           // epilogue thread index
-    const int row = m0 + q * 32 + lane;
-    const size_t grow = (size_t)b * p.NA + min(row, p.NA - 1);
-    // candidate threshold in TMEM units (scores there are true scores * 2^28)
-    const float thr = screen_threshold(__ldg(p.nd_a + grow), __ldg(p.nh_a + grow), __uint_as_float(__ldg(p.nd_b_max)),
-                                       __uint_as_float(__ldg(p.nh_b_max))) * 268435456.0f;
-    float run_m = -INFINITY;
-    int cnt = 0;  // entries appended (only the first SCREEN_K are stored: cnt > SCREEN_K = overflow)
+    // ================= consumers: one hi.hi pass, then the candidate search on the registers =================
+    // Every 16-value chunk (8 column pairs) whose maximum comes within the threshold of the row's running maximum (a
+    // "record" or a near-tie) builds a mask of its qualifying columns and appends their indices to the (thread, row)
+    // list in shared memory.  Values are not kept: a record that beats the previous maximum by more than the threshold
+    // disqualifies the whole list at once (every entry is <= the previous maximum); otherwise the old entries stay -- at
+    // worst a few extra candidates for the exact re-scoring, never a missing one.
+    tc::setmaxnreg_inc<232>();
+    const int wg = (warp >> 2) - 1, qd = lane & 3;
+    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int et = threadIdx.x - 128;  // consumer thread index
+    const uint32_t a_off = (uint32_t)(wg * 64 * 128);
+    float thr[2], run_m[2] = {-INFINITY, -INFINITY};
+    int cnt[2] = {0, 0};  // entries appended (only the first SCREEN_K are stored: cnt > SCREEN_K = overflow)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {  // candidate threshold in accumulator units (scores there are true scores * 2^28)
+      const size_t grow = (size_t)b * p.NA + min(m0 + rl + 8 * h, p.NA - 1);
+      thr[h] = screen_threshold(__ldg(p.nd_a + grow), __ldg(p.nh_a + grow), __uint_as_float(__ldg(p.nd_b_max)),
+                                __uint_as_float(__ldg(p.nh_b_max))) * 268435456.0f;
+    }
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    if (ntiles > 0) tc::mbar_wait(afull, 0);
     for (int t = 0; t < ntiles; ++t) {
-      const int buf = t & 1;
-      tc::mbar_wait(&tfull[buf], (t >> 1) & 1);
-      tc::tc_fence_after();
-      const int colbase = (t0 + t) * BN + half * COLS;
-      if (colbase < p.NB) {  // warp-uniform
-        uint32_t r[COLS / 32][32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN + half * COLS;
-        __syncwarp();
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        tc::mbar_wait(&full[stage], phase);
+        const uint64_t dA = tc::wg_desc_k128(tc::smem_u32(smem + kb * A_BYTES) + a_off);
+        const uint64_t dB = tc::wg_desc_k128(tc::smem_u32(ring + stage * STAGE_BYTES));
+        tc::wg_fence_regs(acc);
+        tc::wg_fence();
 #pragma unroll
-        for (int c = 0; c < COLS / 32; ++c) tc::tmem_ld_32x32(taddr + c * 32, r[c]);
-        tc::tmem_ld_wait();
+        for (int kk = 0; kk < 4; ++kk) tc::wgmma_f16(acc, dA + kk * 2, dB + kk * 2, (kb | kk) ? 1u : 0u);
+        tc::wg_commit();
+        if (prev >= 0) {
+          tc::wg_wait<1>();
+          release_stage<CL>(&empty[prev], lane);
+        }
+        prev = stage;
+        if (++stage == STAGES) stage = 0, phase ^= 1;
+      }
+      tc::wg_wait<0>();
+      tc::wg_fence_regs(acc);
+      release_stage<CL>(&empty[prev], lane);
+
+      const int colbase = (t0 + t) * BN;
 #pragma unroll
-        for (int c = 0; c < COLS / 32; ++c) {
-          const int cb = colbase + c * 32;
-          const int nvalid = p.NB - cb;  // columns at or beyond NB hold zero-filled (TMA) operands: mask them
-          if (nvalid < 32) {
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (i >= nvalid) r[c][i] = __float_as_uint(-INFINITY);
+        for (int c = 0; c < BN / 64; ++c) {  // chunk c: column pairs j = 8c .. 8c+7, bit i <-> (j = 8c + i / 2, e = i % 2)
+          float v[16];
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const int col = colbase + 8 * (8 * c + i / 2) + 2 * qd + (i & 1);
+            // columns at or beyond NB hold zero-filled (TMA) or foreign operands: mask them
+            v[i] = col < p.NB ? acc[4 * (8 * c + i / 2) + 2 * h + (i & 1)] : -INFINITY;
           }
           float cm = -INFINITY;
 #pragma unroll
-          for (int i = 0; i < 32; ++i) cm = fmaxf(cm, __uint_as_float(r[c][i]));
-          if (cm - thr > run_m) cnt = 0;  // a record that disqualifies every earlier entry (all <= the old maximum)
-          run_m = fmaxf(run_m, cm);
-          const float lim = run_m - thr;
+          for (int i = 0; i < 16; ++i) cm = fmaxf(cm, v[i]);
+          if (cm - thr[h] > run_m[h]) cnt[h] = 0;  // a record that disqualifies every earlier entry (all <= the old maximum)
+          run_m[h] = fmaxf(run_m[h], cm);
+          const float lim = run_m[h] - thr[h];
           if (cm >= lim && cm > -INFINITY) {
             uint32_t mask = 0;
 #pragma unroll
-            for (int i = 0; i < 32; ++i) mask |= (__uint_as_float(r[c][i]) >= lim ? 1u : 0u) << i;
+            for (int i = 0; i < 16; ++i) mask |= (v[i] >= lim ? 1u : 0u) << i;
             while (mask) {
               const int i = __ffs(mask) - 1;
               mask &= mask - 1;
-              if (cnt < SCREEN_K) s_ci[cnt * LT + et] = cb + i;
-              ++cnt;
+              if (cnt[h] < SCREEN_K) s_ci[cnt[h] * C::LT + et * 2 + h] = colbase + 8 * (8 * c + i / 2) + 2 * qd + (i & 1);
+              ++cnt[h];
             }
-            if (cnt > SCREEN_K) cnt = SCREEN_K + 1;  // overflow (sticky until a disqualifying record clears the list)
+            if (cnt[h] > SCREEN_K) cnt[h] = SCREEN_K + 1;  // overflow (sticky until a disqualifying record clears the list)
           }
         }
       }
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CL == 1)
-          tc::mbar_arrive(&tempty[buf]);
-        else
-          tc::mbar_arrive_leader(&tempty[buf]);
-      }
     }
-    if (row < p.NA) {
-      const size_t o = ((size_t)(blockIdx.z * SCREEN_HALVES + half) * p.B + b) * p.NA + row;
-      p.pm[o] = run_m * 3.725290298461914e-09f;
-      const bool overflow = cnt > SCREEN_K;
-      if (!overflow)
-        for (int j = 0; j < cnt; ++j) p.pidx[o * SCREEN_K + j] = s_ci[j * LT + et];
-      p.pcnt[o] = overflow ? -1 : cnt;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = m0 + rl + 8 * h;
+      if (row < p.NA) {
+        const size_t o = ((size_t)(blockIdx.z * QUADS + qd) * p.B + b) * p.NA + row;
+        p.pm[o] = run_m[h] * 3.725290298461914e-09f;
+        const bool overflow = cnt[h] > SCREEN_K;
+        if (!overflow)
+          for (int j = 0; j < cnt[h]; ++j) p.pidx[o * SCREEN_K + j] = s_ci[j * C::LT + et * 2 + h];
+        p.pcnt[o] = overflow ? -1 : cnt[h];
+      }
     }
   }
 
-  tc::tc_fence_before();
   __syncthreads();
   if (CL == 2) tc::cluster_sync_all();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    if (CL == 2)
-      tc::tmem_dealloc_pair(tmem_base, 512);
-    else
-      tc::tmem_dealloc(tmem_base, 512);
-  }
 }
+
 
 // Exact re-scoring: one warp per query row.  fp32 dot products of the ORIGINAL fp32 operands (lane l owns dimensions
 // 4l..4l+3 and 128+4l..128+4l+3, eight FMAs, then a butterfly sum that leaves the same bits in every lane), running
@@ -811,12 +661,12 @@ __global__ void __launch_bounds__(256) corr_rescore_kernel(const float* __restri
     const int n = __ldg(p.pcnt + o);
     if (n >= 0) {
       for (int j = 0; j < n; ++j) visit(__ldg(p.pidx + o * SCREEN_K + j));
-    } else {  // overflowed list: every column of the part's range (part = column-range split x column half of each tile)
-      const int sp = s / SCREEN_HALVES, hf = s - sp * SCREEN_HALVES, hc = BN / SCREEN_HALVES;
-      const int tl0 = sp * p.tiles_per_split, tl1 = min((sp + 1) * p.tiles_per_split, ntiles_all);
-      for (int tl = tl0; tl < tl1; ++tl) {
-        const int c0 = tl * BN + hf * hc, c1 = min(c0 + hc, p.NB);
-        for (int col = c0; col < c1; ++col) visit(col);
+    } else {  // overflowed list: every column of the part (column-range split x quad thread: columns with (col / 2) % 4 == qd)
+      const int sp = s / QUADS, qd = s - sp * QUADS;
+      const int c0 = sp * p.tiles_per_split * BN, c1 = min(min((sp + 1) * p.tiles_per_split, ntiles_all) * BN, p.NB);
+      for (int col = c0 + 2 * qd; col < c1; col += 8) {
+        visit(col);
+        if (col + 1 < c1) visit(col + 1);
       }
     }
   }
@@ -911,12 +761,11 @@ int launch_main_cl(const CUtensorMap& mAh, const CUtensorMap& mAl, const CUtenso
                    const TcParams& tp, dim3 grid, cudaStream_t s) {
   static unsigned long long attr_mask = 0;  // the attribute is per device
   if (first_use_on_device(&attr_mask)) {
-    if (cudaFuncSetAttribute(corr_tc_kernel<FMT, SOFTMAX, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<CL>::SMEM_BYTES) !=
-        cudaSuccess)
+    if (cudaFuncSetAttribute(corr_tc_kernel<FMT, SOFTMAX, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES) != cudaSuccess)
       return -1;
   }
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid, cfg.blockDim = dim3(Epi<SOFTMAX>::NTHREADS), cfg.dynamicSmemBytes = Cfg<CL>::SMEM_BYTES, cfg.stream = s;
+  cfg.gridDim = grid, cfg.blockDim = dim3(NTHREADS), cfg.dynamicSmemBytes = Cfg::SMEM_BYTES, cfg.stream = s;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = CL, at[0].val.clusterDim.y = 1, at[0].val.clusterDim.z = 1;
@@ -949,9 +798,9 @@ static size_t screen_cand_bytes(int nparts, int B, int NA) { return (size_t)npar
 int corr_ws_reserve(CorrWorkspace* ws, int B, int Bphi, int NA, int NB) {
   void* d;
   const size_t ea = (size_t)B * NA * 256 * 4, ephi = (size_t)Bphi * NB * 256 * 4;  // tf32 words: the widest format
-  const size_t part = (size_t)16 * 2 * B * NA * sizeof(SplitOut);                   // at most 16 column splits x 2 column halves
+  const size_t part = (size_t)16 * QUADS * B * NA * sizeof(SplitOut);               // at most 16 column splits x 4 quad threads
   if (ws_get(ws, 0, ea, &d) || ws_get(ws, 1, ea, &d) || ws_get(ws, 2, ephi, &d) || ws_get(ws, 3, ephi, &d) || ws_get(ws, 4, part, &d) ||
-      ws_get(ws, 5, screen_norm_bytes(B, Bphi, NA, NB), &d) || ws_get(ws, 6, screen_cand_bytes(16 * SCREEN_HALVES, B, NA), &d))
+      ws_get(ws, 5, screen_norm_bytes(B, Bphi, NA, NB), &d) || ws_get(ws, 6, screen_cand_bytes(16 * QUADS, B, NA), &d))
     return -1;
   return 0;
 }
@@ -968,11 +817,11 @@ template <int CL>
 static int launch_screen_cl(const CUtensorMap& mA, const CUtensorMap& mB, const ScreenParams& sp, dim3 grid, cudaStream_t s) {
   static unsigned long long attr_mask = 0;
   if (first_use_on_device(&attr_mask)) {
-    if (cudaFuncSetAttribute(corr_screen_kernel<CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, ScreenCfg<CL>::SMEM_BYTES) != cudaSuccess)
+    if (cudaFuncSetAttribute(corr_screen_kernel<CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, ScreenCfg::SMEM_BYTES) != cudaSuccess)
       return -1;
   }
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid, cfg.blockDim = dim3(SCREEN_THREADS), cfg.dynamicSmemBytes = ScreenCfg<CL>::SMEM_BYTES, cfg.stream = s;
+  cfg.gridDim = grid, cfg.blockDim = dim3(NTHREADS), cfg.dynamicSmemBytes = ScreenCfg::SMEM_BYTES, cfg.stream = s;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = CL, at[0].val.clusterDim.y = 1, at[0].val.clusterDim.z = 1;
@@ -995,7 +844,10 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
   if (ws_get(ws, 0, ea * eb, &Ah) || ws_get(ws, 1, ea * eb, &Al) || ws_get(ws, 2, ephi * eb, &Bh) || ws_get(ws, 3, ephi * eb, &Bl))
     return fail("workspace allocation failed");
 
-  // column-range splits so that (row blocks x batch x splits) fills the 148 SMs in whole waves
+  int dev = 0, num_sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return fail("cudaDeviceGetAttribute(multiProcessorCount) failed");
+  // column-range splits so that (row blocks x batch x splits) fills the SMs in whole waves
   const int cl = cluster == 2 ? 2 : 1;
   const int row_blocks = ((p.NA + BM - 1) / BM + cl - 1) / cl * cl;  // pairs: an even number of 128-row query tiles
   const int ntiles = (p.NB + BN - 1) / BN;
@@ -1007,8 +859,8 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
       const int tps = (ntiles + sp - 1) / sp;
       const int eff_sp = (ntiles + tps - 1) / tps;
       const long total = ctas * eff_sp;
-      const long waves = (total + 147) / 148;
-      const double eff = (double)total / (double)(waves * 148) * ((double)ntiles / (double)(tps * eff_sp)) -
+      const long waves = (total + num_sms - 1) / num_sms;
+      const double eff = (double)total / (double)(waves * num_sms) * ((double)ntiles / (double)(tps * eff_sp)) -
                          0.01 * sp;  // mild penalty: every split re-runs the prologue
       if (eff > best) best = eff, nsplit = eff_sp;
     }
@@ -1020,7 +872,7 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
     // ---- screened T -> 0 path: hi planes + error norms, one fp16 pass, exact re-scoring of the candidates ----
     const int rows = p.B * p.NA, rphi = p.Bphi * p.NB;
     void *norms, *cand;
-    const int sparts = nsplit * SCREEN_HALVES;
+    const int sparts = nsplit * QUADS;
     if (ws_get(ws, 5, screen_norm_bytes(p.B, p.Bphi, p.NA, p.NB), &norms) || ws_get(ws, 6, screen_cand_bytes(sparts, p.B, p.NA), &cand))
       return fail("workspace allocation failed");
     float* nd_a = (float*)norms;
@@ -1052,10 +904,10 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
     launch_counter_add(2);
     return 0;
   }
-  const int nparts = nsplit * Epi<true>::HALVES;  // partial rows the merge kernel combines
+  const int nparts = nsplit * QUADS;  // partial rows the merge kernel combines
   if (ws_get(ws, 4, (size_t)nparts * p.B * p.NA * sizeof(SplitOut), &part)) return fail("workspace allocation failed");
 
-  const int grid1 = 148 * 8;
+  const int grid1 = num_sms * 8;
   // the reference side's planes survive from launch to launch while (pointer, version, format, size) are unchanged
   const bool phi_cached = phi_version >= 0 && ws->phi_src == p.phi && ws->phi_version == phi_version && ws->phi_fmt == fmt &&
                           ws->phi_elems == ephi;

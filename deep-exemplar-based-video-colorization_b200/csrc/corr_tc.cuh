@@ -1,4 +1,4 @@
-// tcgen05 (5th-gen tensor core) implementation of K7; see corr_tc.cu.
+// Hopper tensor-core (wgmma) implementation of K7; see corr_tc.cu.
 #pragma once
 #include <string>
 
@@ -22,7 +22,7 @@ struct CorrWorkspace {
 int corr_ws_reserve(CorrWorkspace* ws, int B, int Bphi, int NA, int NB);
 void corr_ws_free(CorrWorkspace* ws);
 // math = DVC_MATH_TF32X3 / BF16X3 / FP16X3.  Returns 0 on success, non-zero with *err set otherwise.
-// cluster: 2 = CTA pairs (tcgen05.mma.cta_group::2) on adjacent query-row tiles, 1 = single CTAs
+// cluster: 2 = 2-CTA clusters on adjacent query-row tiles sharing the multicast reference tile, 1 = single CTAs
 // phi_version >= 0: the caller guarantees that p.phi's contents change only together with phi_version (the planes of
 // the reference side are then reused across launches); < 0: split every launch
 // screen != 0 (FP16X3, T <= 2e-10 only): one fp16 pass locates the candidates of every row's maximum within a rigorous error

@@ -120,14 +120,14 @@ struct dvc_ctx {
   std::unordered_map<std::string, float> slope[3];
   std::unordered_map<std::string, float*> vec[3];
   std::unordered_map<std::string, std::vector<float>> host_bias[3];  // bias seen before its weight
-  int num_sms = 148;
+  int num_sms = 132;
   // default: tensor cores with fp32-class accuracy (3xTF32); DVC_MATH_FP32 selects the exact CUDA-core engines
   int conv_math = DVC_MATH_TF32X3, corr_math = DVC_MATH_FP16X3;
   int tc_kbytes = 128;    // tensor-core convolutions: K bytes per pipeline stage (64 or 128, see conv_tc.cu)
   CorrPeers corr_peers;   // fused all-gather targets of dvc_corr_softmax_warp (dvc_corr_set_peer_outputs)
   ScaleCell* cell_next = nullptr;
   int cell_left = 0;
-  int corr_cluster = 2;   // correlation: 2 = CTA pairs (tcgen05.mma.cta_group::2), 1 = single CTAs
+  int corr_cluster = 2;   // correlation: 2 = 2-CTA clusters sharing the multicast reference tile, 1 = single CTAs
   // stand-alone correlation entry: the caller promises that the phi_hat / V buffers keep their contents while this is set, so
   // their transposed / packed / split forms are prepared once per (pointer, size) -- the exemplar side of a clip
   int corr_phi_static = 0;
@@ -146,8 +146,8 @@ struct dvc_ctx {
                           // launches (-1.3 % on one stream, +1.6 % in the two-stream clip pipeline: off by default)
   int tc_f16 = 1;         // tensor-core convolutions: fp16 hi/lo planes for layers with provably bounded inputs
   std::unordered_map<std::string, float> vec_absmax[3];  // max |scale| of the *_ss vectors
-  int tc_cluster = 2;     // tensor-core convolutions: 2 = CTA pairs (tcgen05.mma.cta_group::2), 1 = single CTAs
-  int tc_kc = 1;          // tensor-core convolutions: k-blocks per TMEM chunk (see conv_tc.cu)
+  int tc_cluster = 2;     // tensor-core convolutions: 2 = 2-CTA clusters sharing the multicast weight tile, 1 = single CTAs
+  int tc_kc = 1;          // tensor-core convolutions: k-blocks per accumulator chunk (see conv_tc.cu)
   bool two_level = true;  // fp32 convolutions: per-tap two-level accumulation (see conv_simt.cu)
   std::map<std::string, Buf> bufs;
   // InstanceNorm statistics arena (doubles), bump-allocated per forward call
@@ -1046,7 +1046,7 @@ static int colorvid(dvc_ctx* c, const std::string& tag, const Act& in0, float* o
 // ------------------------------------------------------------------------------------------------
 static bool legal_shape(int H, int W) { return H >= 16 && W >= 16 && H % 8 == 0 && W % 16 == 0; }
 
-extern "C" const char* dvc_version(void) { return "libdvc 0.1 (sm_100a)"; }
+extern "C" const char* dvc_version(void) { return "libdvc 0.1 (sm_90a)"; }
 
 extern "C" int dvc_create(dvc_ctx** out, int device) {
   if (!out) return DVC_ERR_ARG;
@@ -1068,8 +1068,8 @@ extern "C" int dvc_create(dvc_ctx** out, int device) {
   }
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
-  if (prop.major != 10) {
-    g_create_err = "libdvc is built for sm_100a only; device is sm_" + std::to_string(prop.major * 10 + prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    g_create_err = "libdvc is built for sm_90a only; device is sm_" + std::to_string(prop.major * 10 + prop.minor);
     return DVC_ERR_CUDA;
   }
   dvc_ctx* c = new dvc_ctx();

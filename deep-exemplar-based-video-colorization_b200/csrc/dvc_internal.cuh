@@ -1,6 +1,6 @@
 // Internal declarations shared by the kernels and the host-side layer programs of libdvc.so.
 //
-// Data layout in HBM (DESIGN.md §3): every activation is a "padded NHWC" fp32 tensor
+// Data layout in HBM: every activation is a "padded NHWC" fp32 tensor
 //     [B][H + 2P][W + 2P][C]
 // whose border of width P already holds what the consumer's padding mode would produce (zeros for
 // the VGG / ColorVidNet convolutions, mirrored pixels for WarpNet's ReflectionPad2d).  With that

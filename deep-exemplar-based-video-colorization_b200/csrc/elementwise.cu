@@ -601,7 +601,7 @@ __global__ void __launch_bounds__(256) upsample2_kernel(const float* __restrict_
   }
 }
 
-inline int grid_for(long total, int threads, int cap = 148 * 16) {
+inline int grid_for(long total, int threads, int cap = 132 * 16) {
   long g = (total + threads - 1) / threads;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
@@ -670,7 +670,7 @@ void launch_maxpool2_h16(const void* h16, const void* l16, const ScaleCell* cell
 }
 
 void launch_amax(const float* x, size_t n, ScaleCell* cell, cudaStream_t s) {
-  amax_kernel<<<(unsigned)grid_for((long)(n / 4), 256, 148 * 4), 256, 0, s>>>(reinterpret_cast<const float4*>(x), n / 4, cell);
+  amax_kernel<<<(unsigned)grid_for((long)(n / 4), 256, 132 * 4), 256, 0, s>>>(reinterpret_cast<const float4*>(x), n / 4, cell);
   launch_counter_add(1);
 }
 

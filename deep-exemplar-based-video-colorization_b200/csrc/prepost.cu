@@ -281,7 +281,7 @@ __global__ void __launch_bounds__(256) ctx_loss_kernel(const float* __restrict__
   if (threadIdx.x == 0) loss[blockIdx.x] = (float)(-log(red[0] / N));
 }
 
-inline int grid_for(size_t total, int threads, int cap = 148 * 16) {
+inline int grid_for(size_t total, int threads, int cap = 132 * 16) {
   const size_t g = (total + threads - 1) / threads;
   return (int)(g < (size_t)cap ? (g ? g : 1) : cap);
 }

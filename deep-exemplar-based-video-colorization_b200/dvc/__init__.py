@@ -1,7 +1,7 @@
 """ctypes binding of libdvc.so (include/dvc.h) -- the only way Python reaches the CUDA kernels.
 
 PyTorch is used for device memory, streams and torch.distributed; every FLOP of the hot path runs
-in hand-written sm_100a kernels inside libdvc.so.  There is no CPU fallback and no torch fallback:
+in hand-written sm_90a kernels inside libdvc.so.  There is no CPU fallback and no torch fallback:
 if the library or a CUDA device is missing, every entry point raises.
 """
 import ctypes

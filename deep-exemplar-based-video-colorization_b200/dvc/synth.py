@@ -2,7 +2,7 @@
 
 Used by bench.py, __graft_entry__.smoke() and (through oracle/weights.py) by the tests: the CUDA path and the
 CPU oracle must see the very same tensors.  Pretrained checkpoints are not in the reference tree
-(/root/reference/.gitignore:4 excludes *.pth) and cannot be downloaded, so every parity
+(the reference's .gitignore:4 excludes *.pth) and cannot be downloaded, so every parity
 test uses seeded random weights.  The generator below does not depend on module
 construction order or on the global RNG: each tensor is drawn from its own
 `torch.Generator` seeded with (seed, index-of-key), which makes the result identical in

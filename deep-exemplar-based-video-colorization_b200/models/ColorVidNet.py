@@ -1,4 +1,4 @@
-"""B200-native drop-in for `models.ColorVidNet.ColorVidNet` (/root/reference/models/ColorVidNet.py:6-144).
+"""H100-native drop-in for `models.ColorVidNet.ColorVidNet` (the reference's models/ColorVidNet.py:6-144).
 
 Same constructor / forward signature and the same 65 state_dict keys; forward() runs the 34-conv
 encoder-decoder (InstanceNorm x9, dilated middle, three skip adds, tanh*128) in libdvc.so.
@@ -44,7 +44,7 @@ class ColorVidNet(nn.Module):
 
     def forward(self, x):
         if not x.is_cuda:
-            raise dvc.DvcError("the B200 drop-in modules run on CUDA tensors only (no CPU fallback)")
+            raise dvc.DvcError("the H100 drop-in modules run on CUDA tensors only (no CPU fallback)")
         ctx = dvc.get_context(x.device.index)
         ctx.sync_module_weights(dvc.NET_COLOR, self)
         return ctx.colorvidnet_forward(x)

@@ -1,9 +1,9 @@
-"""B200-native drop-ins for `models.NonlocalNet.VGG19_pytorch` and `models.NonlocalNet.WarpNet`.
+"""H100-native drop-ins for `models.NonlocalNet.VGG19_pytorch` and `models.NonlocalNet.WarpNet`.
 
 Same constructor / forward signatures and state_dict keys as the reference
-(/root/reference/models/NonlocalNet.py:192-256 and 355-502) so that the reference's test.py and
+(the reference's models/NonlocalNet.py:192-256 and 355-502) so that the reference's test.py and
 models/FrameColor.py run unchanged with this directory ahead of the reference on sys.path.  The
-forward passes call hand-written sm_100a kernels in libdvc.so through ctypes (dvc/__init__.py);
+forward passes call hand-written sm_90a kernels in libdvc.so through ctypes (dvc/__init__.py);
 there is no torch fallback and no CPU path.
 """
 import torch
@@ -23,7 +23,7 @@ _COMPARE = __import__("os").environ.get("DVC_DROPIN_COMPARE", "1") != "0"
 
 def _ctx_for(t):
     if not t.is_cuda:
-        raise dvc.DvcError("the B200 drop-in modules run on CUDA tensors only (no CPU fallback); call .cuda() like test.py:164-166")
+        raise dvc.DvcError("the H100 drop-in modules run on CUDA tensors only (no CPU fallback); call .cuda() like test.py:164-166")
     return dvc.get_context(t.device.index)
 
 

@@ -1,5 +1,5 @@
 /*
- * libdvc.so -- C ABI of the B200-native exemplar-video-colorization forward path.
+ * libdvc.so -- C ABI of the H100-native exemplar-video-colorization forward path.
  *
  * The reference (zhangmozhe/Deep-Exemplar-based-Video-Colorization) has no FFI of its own: its
  * hot path is three Python nn.Module.forward() methods plus per-frame glue.  Each entry point below
@@ -44,10 +44,10 @@ typedef enum dvc_net { DVC_NET_VGG = 0, DVC_NET_WARP = 1, DVC_NET_COLOR = 2 } dv
 
 /* Arithmetic used by the GEMM-shaped kernels (convolutions, correlation).
  *   DVC_MATH_FP32    CUDA-core fp32 FMA (exact fp32 products, two-level accumulation; the on-GPU fp32 reference)
- *   DVC_MATH_TF32X3  tcgen05 kind::tf32 on hi/lo split operands, 3 MMAs per product, TMEM chunk sums promoted
+ *   DVC_MATH_TF32X3  wgmma tf32 on hi/lo split operands, 3 MMAs per product, accumulator chunk sums promoted
  *                    to fp32 registers (fp32-class accuracy; THE DEFAULT for convolutions and correlation)
- *   DVC_MATH_BF16X3  tcgen05 kind::f16 (bf16) on hi/lo split operands (correlation only; fast mode, |df| ~ 2e-6)
- *   DVC_MATH_FP16X3  tcgen05 kind::f16 (fp16) on hi/lo planes of x * 2^14 (correlation only: its operands are unit
+ *   DVC_MATH_BF16X3  wgmma bf16 on hi/lo split operands (correlation only; fast mode, |df| ~ 2e-6)
+ *   DVC_MATH_FP16X3  wgmma fp16 on hi/lo planes of x * 2^14 (correlation only: its operands are unit
  *                    vectors, so the power-of-two scale is exact): tf32x3's 2 x 11 bits at bf16x3's speed
  */
 typedef enum dvc_math { DVC_MATH_FP32 = 0, DVC_MATH_TF32X3 = 1, DVC_MATH_BF16X3 = 2, DVC_MATH_FP16X3 = 3 } dvc_math;

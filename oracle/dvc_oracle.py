@@ -4,19 +4,19 @@ Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl refere
 import this file; the product (libdvc.so and the drop-in modules) never does.
 
 What this is: a functional, parameter-dict restatement of the reference's forward path,
-  /root/reference/models/FrameColor.py:5-67      (warp_color, frame_colorization)
-  /root/reference/models/NonlocalNet.py:228-256  (VGG19_pytorch.forward)
-  /root/reference/models/NonlocalNet.py:330-352  (ResidualBlock.forward)
-  /root/reference/models/NonlocalNet.py:427-502  (WarpNet.forward)
-  /root/reference/models/ColorVidNet.py:96-144   (ColorVidNet.forward)
-  /root/reference/utils/util.py:63,97-101,155-158,347-352,379-414 (helpers)
+  models/FrameColor.py:5-67      (warp_color, frame_colorization)
+  models/NonlocalNet.py:228-256  (VGG19_pytorch.forward)
+  models/NonlocalNet.py:330-352  (ResidualBlock.forward)
+  models/NonlocalNet.py:427-502  (WarpNet.forward)
+  models/ColorVidNet.py:96-144   (ColorVidNet.forward)
+  utils/util.py:63,97-101,155-158,347-352,379-414 (helpers)
 written against torch CPU ops (the arithmetic of the reference lives in PyTorch, a
 third-party dependency that requirements.txt:11 leaves unpinned; this container's torch
 2.11.0 is the de-facto pinned version).  Every function is dtype-generic: pass fp32
 parameters/inputs for the "reference fp32" oracle and fp64 for the "truth" oracle.
 
-Pinning: oracle/make_golden.py imports the real reference modules from /root/reference (in the
-build container only), runs both on the same seeded weights/inputs, asserts agreement and
+Pinning: oracle/make_golden.py imports the real reference modules from a checkout of the
+reference named by DVC_REFERENCE_ROOT, runs both on the same seeded weights/inputs, asserts agreement and
 writes tests/golden/*.npz.  tests/test_oracle_golden.py re-checks this file against those
 vectors on every run (CPU).  The reference itself ships no tests and no golden vectors
 (SURVEY.md §4), so these generated vectors are the only pin available.

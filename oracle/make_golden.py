@@ -2,8 +2,8 @@
 
     python oracle/make_golden.py            # writes tests/golden/, prints the pin report
 
-For every case the real reference modules (imported read-only from /root/reference through
-oracle/ref_import.py) run `frame_colorization` on seeded weights (oracle/weights.py) and seeded
+For every case the real reference modules (imported read-only from the checkout named by
+DVC_REFERENCE_ROOT through oracle/ref_import.py) run `frame_colorization` on seeded weights (oracle/weights.py) and seeded
 inputs in fp32 (the reference's own arithmetic) and in fp64 (same modules, .double()).  The
 restatement in oracle/dvc_oracle.py is run on the same tensors and must agree BIT-EXACTLY with
 the fp32 reference (same torch ops in the same order) -- that is the pin.  What is stored:

@@ -1,6 +1,6 @@
-"""Import the UNMODIFIED reference modules from /root/reference (build container only).
+"""Import the UNMODIFIED reference modules from a checkout of the reference named by DVC_REFERENCE_ROOT.
 
-TEST INFRASTRUCTURE.  /root/reference does not exist on the GPU box, so nothing under
+TEST INFRASTRUCTURE.  The reference is not part of this repository, so nothing under
 `-m gpu`, smoke() or bench.py may call this; it is used by oracle/make_golden.py (fixture
 generation) and by the CPU-only test that pins oracle/dvc_oracle.py to the reference when the
 tree is present.
@@ -15,11 +15,11 @@ import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("DVC_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("DVC_REFERENCE_ROOT", "")
 
 
 def available():
-    return os.path.isfile(os.path.join(REF_ROOT, "models", "NonlocalNet.py"))
+    return bool(REF_ROOT) and os.path.isfile(os.path.join(REF_ROOT, "models", "NonlocalNet.py"))
 
 
 def load():

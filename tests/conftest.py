@@ -13,7 +13,7 @@ GOLD = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
 
 
 @pytest.fixture(scope="session")
@@ -36,7 +36,7 @@ def ctx(sds):
     c.set_weights(dvc.NET_VGG, sds["vgg"])
     c.set_weights(dvc.NET_WARP, sds["warp"])
     c.set_weights(dvc.NET_COLOR, sds["color"])
-    if os.environ.get("DVC_TEST_KC"):  # parity of a coarser TMEM promotion chunk (DESIGN.md, precision findings)
+    if os.environ.get("DVC_TEST_KC"):  # parity of a coarser accumulator promotion chunk (conv_tc.cu)
         c.debug_flag("tc_kc", int(os.environ["DVC_TEST_KC"]))
     return c
 

@@ -31,7 +31,7 @@ def run(H, W, seed, tl):
     ctx.set_exemplar(IB)
     ab, warp, sim = ctx.colorize_frames(IA[:, 0:1].cuda(), last.cuda(), 1e-10, want_warp=True)
     N = (H // 4) * (W // 4)
-    print(f"  (mode {tl}: 0 plain fp32, 1 two-level fp32, 2x tcgen05 tf32x3 with kc = x)")
+    print(f"  (mode {tl}: 0 plain fp32, 1 two-level fp32, 2x wgmma tf32x3 with kc = x)")
     th = ctx.debug_buffer("fr.theta", act=False)[: N * 256].view(N, 256).t().cpu().double()
     ph = ctx.debug_buffer("ex.phi", act=False)[: N * 256].view(N, 256).t().cpu().double()
     e_th = (th - ex64["theta_hat"][0]).abs().max().item(); e_th32 = (ex32["theta_hat"][0].double() - ex64["theta_hat"][0]).abs().max().item()

@@ -1,4 +1,4 @@
-"""Per-layer parity of the convolution engines (run with -m gpu on a B200): ONE nn.Conv2d of the reference
+"""Per-layer parity of the convolution engines (run with -m gpu on an H100): ONE nn.Conv2d of the reference
 (NonlocalNet.py:235-255,364-423; ColorVidNet.py:96-143) through dvc_debug_conv2d -- the same engine, operand planes and
 epilogue the layer programs use -- against F.conv2d evaluated in float64 on the CPU with the same seeded weights.
 
@@ -149,11 +149,11 @@ def test_layer_batch2_tiles_straddle_images(ctx, sds, engine):
 
 # ---- the bench's own geometry (480x864 frame: 120x216 quarter-resolution, 60x108 eighth-resolution maps) ----
 BENCH = [
-    # 104 pair items on 74 pair slots: the launcher's cost model takes three rounds of 128-channel tiles over two of 256
+    # layers with more than 64 output channels run on the 128 x 128 tile unless another tile is forced (conv_tc.cu)
     ("quarter_256_208tiles", VGG, "conv3_2", 256, 256, 120, 216, dict(act=1, nonneg=True), 128),
     ("quarter_256_reflect_stats", WARP, "layer.0.conv1", 256, 256, 120, 216, dict(reflect=True, want_stats=True), 128),
-    ("eighth_512_108tiles", VGG, "conv4_2", 512, 512, 60, 108, dict(act=1, nonneg=True), 256),
-    ("eighth_512_dil2_stats", COLOR, "conv5_3", 512, 512, 60, 108, dict(act=1, dil=2, nonneg=True, want_stats=True), 256),
+    ("eighth_512_108tiles", VGG, "conv4_2", 512, 512, 60, 108, dict(act=1, nonneg=True), 128),
+    ("eighth_512_dil2_stats", COLOR, "conv5_3", 512, 512, 60, 108, dict(act=1, dil=2, nonneg=True, want_stats=True), 128),
     ("half_128", VGG, "conv2_2", 128, 128, 240, 432, dict(act=1, nonneg=True), 128),
     # the four phases of conv8_1 each see 54 pixel tiles of the 1/8-resolution input: the launcher narrows to 128 channels
     ("quarter_upconv_256", COLOR, "conv8_1.1", 512, 256, 60, 108, dict(act=1, upconv=True, with_add=True), 128),
@@ -163,7 +163,7 @@ BENCH = [
 @pytest.mark.parametrize("force_bn", [256, 128])
 @pytest.mark.parametrize("layer", BENCH[:4], ids=[l[0] for l in BENCH[:4]])
 def test_layer_at_bench_geometry_forced_tile(ctx, sds, layer, force_bn):
-    """Both candidate tiles of the launcher's cost model at the bench's geometry (two rounds of 256 / three of 128)."""
+    """The 64 x 256 and 128 x 128 tiles at the bench's geometry."""
     import dvc
 
     _, net, name, cin, cout, H, W, kw, _ = layer

@@ -1,10 +1,10 @@
-"""Oracle parity AT the headline configuration (run with -m gpu on a B200).
+"""Oracle parity AT the headline configuration (run with -m gpu on an H100).
 
 BASELINE.json configs[1] (480x854 padded to 480x864, N = 25920 positions -- the size bench.py measures) and configs[0]
 (256x256), against golden outputs of the UNMODIFIED reference run in fp32 and fp64 by oracle/make_golden.py
 (tests/golden/default_480x864.npz, cfg1_256x256.npz; the inputs are regenerated from the stored seed).  At this size the
-launcher picks the 256-channel CTA-pair tiles, the 208-tile two-round layers and the 204 x 5 correlation grid, none of
-which the small goldens reach.
+launcher runs the 512-channel layers on 128-channel tiles over more than one round of 2-CTA clusters and the correlation
+on a multi-split grid, neither of which the small goldens reach.
 
 Gates (SURVEY.md §8c): similarity |d| < 2e-5; tie-aware argmax (rows whose fp64 top-2 gap > 1e-5 must warp to the
 fp64 colour); ab within max(1e-3, 1.25 x floor) of the fp64 reference, where floor = |ab32_tf - ab64| is the reference's
@@ -53,11 +53,11 @@ def test_fused_frame_vs_reference_at_full_size(ctx, engine, name, H, W):
     ab, warp, sim = ctx.colorize_frames(IA[:, 0:1].cuda(), last.cuda(), T, want_warp=True)
     torch.cuda.synchronize()
     if engine == "tf32x3":
-        n256 = ctx.conv_profile(256)[0]
+        n128 = ctx.conv_profile(128)[0]
         ctx.conv_profile(0, reset=True)
         ctx.profile_conv(False)
-        if H == 480:  # the sixteen 1/8-resolution 512-channel layers (the quarter-resolution ones take 128-channel tiles)
-            assert n256 >= 12, f"only {n256} launches ran on the 256-channel tile: this test must cover the bench's engine"
+        if H == 480:  # the 1/8-resolution 512-channel layers among them
+            assert n128 >= 12, f"only {n128} launches ran on the 128-channel tile: this test must cover the bench's engine"
     ss = sim.cpu().numpy()[:, :, ::4, ::4]
     ys = warp.cpu().numpy()[:, :, ::4, ::4].reshape(1, 3, -1)
     e_sim = np.abs(ss - g["sim64"]).max()

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA path through the C ABI against
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path through the C ABI against
 (1) the committed golden vectors generated from the real reference, (2) the CPU oracle run here on the
 same seeded inputs, (3) size-independent properties at the full 480x864 bench size.
 
@@ -7,7 +7,7 @@ Tolerances (floating point, stated per SURVEY.md §8c):
   similarity      max|d| <= 2e-5
   warp (T->0)     identical argmax on every row whose fp64 top-2 gap > 1e-5 (tie-aware)
   final ab        max|ours - ref_fp64| <= max(1e-3, k * max|ref_fp32 - ref_fp64|): ColorVidNet with the seeded
-                  random weights amplifies a 1e-6 input perturbation to ~1e-3 (measured, DESIGN.md), so the
+                  random weights amplifies a 1e-6 input perturbation to ~1e-3 (measured against the fp64 oracle), so the
                   reference's own fp32 forward sits 1e-3..2e-2 away from fp64; ours must be in the same band.
                   k = 1.25 (SURVEY.md §8c) for the default engine and the exact-fp32 CUDA-core engine; k = 2 only for
                   the debug variants of the tensor-core engine (single CTAs, 64-byte stages, split-K, tail rounds,
@@ -41,12 +41,11 @@ def ab_gate(ours, g, variant="debug"):
 @pytest.fixture(params=["fp32", "tf32x3", "tf32x3-bn256", "tf32x3-bn256-cluster1", "tf32x3-bn64", "tf32x3-nof16", "tf32x3-cluster1",
                         "tf32x3-cluster1-nof16", "tf32x3-cluster1-k64", "tf32x3-k64", "tf32x3-split3", "tf32x3-tail16", "tf32x3-tail"])
 def conv_math(request, ctx):
-    """Convolutions on CUDA cores (exact fp32, two-level accumulation) and on tcgen05 (3xTF32 operand split),
-    the latter as single CTAs (64-byte and 128-byte K stages) and as CTA pairs (tcgen05.mma.cta_group::2).
+    """Convolutions on CUDA cores (exact fp32, two-level accumulation) and on wgmma (3xTF32 operand split),
+    the latter as single CTAs (64-byte and 128-byte K stages) and as 2-CTA clusters (multicast weight tiles).
     Layers with provably bounded inputs run 3xFP16 on scaled planes unless "-nof16" turns that off.
-    "-bn256" pins the 256-channel tile (BN = 256: its own TMEM ring depth, stage count and two-loads-in-flight drain) on
-    every layer with >= 256 output channels -- the tile the 480x864 bench runs on, which the launcher's heuristic
-    never picks at the golden sizes; "-bn64" pins the narrow tile on every layer."""
+    "-bn256" pins the 64 x 256 tile (two warpgroups split the channels; its own stage count) on every layer with >= 256
+    output channels, which the launcher never picks by itself; "-bn64" pins the narrow tile on every layer."""
     import dvc
 
     if request.param.startswith("tf32x3"):
@@ -99,8 +98,8 @@ def test_vgg19_all_keys_and_no_preprocess(ctx, conv_math, sds):
 @pytest.fixture(params=["fp32", "tf32x3", "bf16x3", "fp16x3", "tf32x3-single", "fp16x3-single", "fp16x3-noscreen",
                         "fp16x3-noscreen-single"])
 def corr_math(request, ctx):
-    """Run the correlation tests on the CUDA-core kernel and on the tcgen05 operand-split modes, as CTA pairs
-    (cta_group::2, the default) and as single CTAs.  fp16x3 at T -> 0 takes the screened path by default (one fp16 pass
+    """Run the correlation tests on the CUDA-core kernel and on the wgmma operand-split modes, as 2-CTA clusters
+    (multicast reference tiles, the default) and as single CTAs.  fp16x3 at T -> 0 takes the screened path by default (one fp16 pass
     + exact fp32 re-scoring of the candidates); "-noscreen" pins the exact 3-pass kernel."""
     import dvc
 
@@ -393,7 +392,7 @@ def test_fused_clip_recurrence(ctx, conv_math):
         assert torch.equal(ab.cpu(), out[t:t + 1])
         last = torch.cat((L, ab), 1)
     # free-running against the reference's free-running clip: frame 0 has no history and must match; afterwards the
-    # recurrence is chaotic (DESIGN.md §2: two bit-different fp32 runs of the REFERENCE are 0.4 apart by frame 3, its 1- vs
+    # recurrence is chaotic (two bit-different fp32 runs of the REFERENCE are 0.4 apart by frame 3, its 1- vs
     # 8-thread runs 1.5e-3 apart on a single frame), so the later frames are reported, not gated
     free = [float(np.abs(out[t].numpy() - ref[t]).max()) for t in range(frames.shape[0])]
     print(f"free-running |ab - reference| per frame ({conv_math}): " + ", ".join(f"{v:.2e}" for v in free))

@@ -1,7 +1,7 @@
 """Row-shared taps of the tensor-core convolution engine (conv_tc.cu: CfgRS): the three horizontal taps of a 3x3 row read
 one activation tile through descriptors that start a few rows apart.  Per-layer parity against an fp64 F.conv2d and the
 network goldens, in both descriptor variants (debug flag tc_rowshare = 1: plain shifted start address, 2: shifted start
-address + the descriptor's base-offset field).  Run with -m gpu on a B200."""
+address + the descriptor's base-offset field).  Run with -m gpu on an H100."""
 import os
 
 import numpy as np

@@ -151,30 +151,54 @@ def test_exemplar_broadcast_world2_gloo(tmp_path):
         assert p.returncode == 0 and "OK" in o, o
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/models"), reason="reference tree not present (GPU box)")
-def test_dropin_import_resolution_with_reference_tree():
+def _reference_shaped_tree(root):
+    """The layout of the reference that the import resolution depends on: `models/` WITHOUT an __init__.py (a namespace
+    package) holding NonlocalNet.py, ColorVidNet.py and FrameColor.py, plus utils/ and test.py at the root."""
+    models = root / "models"
+    models.mkdir(parents=True)
+    (models / "NonlocalNet.py").write_text("class VGG19_pytorch: pass\nclass WarpNet: pass\nREFERENCE_FILE = True\n")
+    (models / "ColorVidNet.py").write_text("class ColorVidNet: pass\nREFERENCE_FILE = True\n")
+    (models / "FrameColor.py").write_text("from utils.util import feature_normalize\n\n\ndef frame_colorization(*args, **kwargs):\n    pass\n")
+    (root / "utils").mkdir()
+    (root / "utils" / "util.py").write_text("def feature_normalize(x):\n    return x\n")
+    (root / "test.py").write_text("from models.NonlocalNet import VGG19_pytorch, WarpNet\nfrom models.ColorVidNet import ColorVidNet\n")
+    return str(root)
+
+
+@pytest.mark.parametrize("tree", ["reference_shaped", "live_reference"])
+def test_dropin_import_resolution_with_reference_tree(tmp_path, tree):
     """INTEGRATION.md §1: with the package ahead of the reference on sys.path, `models.NonlocalNet` /
-    `models.ColorVidNet` are the drop-ins while `models.FrameColor` is still the reference's own file."""
+    `models.ColorVidNet` are the drop-ins while `models.FrameColor` is still the reference's own file.  Checked on a
+    reference-shaped tree built here, and on the unmodified reference when its checkout is present (DVC_REFERENCE_ROOT)."""
+    from oracle import ref_import
+
+    if tree == "live_reference":
+        if not ref_import.available():
+            pytest.skip("no checkout of the reference (DVC_REFERENCE_ROOT)")
+        ref_root = os.path.abspath(ref_import.REF_ROOT)
+    else:
+        ref_root = _reference_shaped_tree(tmp_path / "reference")
     code = r"""
-import sys, types
+import os, sys, types
 for n in ["matplotlib", "matplotlib.pyplot", "skimage", "skimage.color", "skimage.io"]:
     sys.modules.setdefault(n, types.ModuleType(n))
 sys.modules["matplotlib"].pyplot = sys.modules["matplotlib.pyplot"]
 sys.modules["skimage"].color = sys.modules["skimage.color"]; sys.modules["skimage"].io = sys.modules["skimage.io"]
-sys.path.insert(0, "/root/reference"); sys.path.insert(0, sys.argv[1])
+ref = sys.argv[2]
+sys.path.insert(0, ref); sys.path.insert(0, sys.argv[1])
 import models
-models.__path__.append("/root/reference/models")
+models.__path__.append(os.path.join(ref, "models"))
 from models.NonlocalNet import VGG19_pytorch, WarpNet
 from models.ColorVidNet import ColorVidNet
 from models.FrameColor import frame_colorization
-import models.NonlocalNet as N, models.FrameColor as F
-assert sys.argv[1] in N.__file__, N.__file__
-assert F.__file__.startswith("/root/reference/"), F.__file__
-assert "dvc" in N.__dict__            # the drop-in imports the ctypes binding, the reference's file does not
+import models.NonlocalNet as N, models.ColorVidNet as C, models.FrameColor as F
+assert sys.argv[1] in N.__file__ and sys.argv[1] in C.__file__, (N.__file__, C.__file__)
+assert F.__file__.startswith(ref + os.sep), F.__file__
+assert "dvc" in N.__dict__ and "dvc" in C.__dict__   # the drop-ins import the ctypes binding, the reference's files do not
 print("RESOLVED")
 """
     pkg = os.path.join(ROOT, "deep-exemplar-based-video-colorization_b200")
-    out = subprocess.run([sys.executable, "-c", code, pkg], capture_output=True, text=True, timeout=120)
+    out = subprocess.run([sys.executable, "-c", code, pkg, ref_root], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0 and "RESOLVED" in out.stdout, out.stdout + out.stderr
 
 

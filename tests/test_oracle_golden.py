@@ -57,7 +57,7 @@ def test_oracle_intermediates_small(sds):
 
 def test_oracle_clip_recurrence(sds):
     """test.py:76-96: with teacher forcing (the reference's own previous prediction as `last`) every frame
-    matches; the free-running recurrence is chaotic with random weights (see DESIGN.md) and is checked
+    matches; the free-running recurrence is chaotic with random weights and is checked
     only for plumbing (first frame starts from zeros)."""
     g = load_golden("clip3_32x48")
     frames, IB, ref = torch.from_numpy(g["frames_lab"]), torch.from_numpy(g["IB_lab"]), torch.from_numpy(g["ab32"])
@@ -81,7 +81,7 @@ def test_chunked_correlation_equals_unchunked():
         assert torch.allclose(y1, y2, atol=1e-5) and torch.allclose(s1, s2, atol=1e-6)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not present (GPU box)")
+@pytest.mark.skipif(not ref_import.available(), reason="no checkout of the reference (DVC_REFERENCE_ROOT)")
 def test_oracle_bit_exact_against_live_reference(sds):
     """In the build container: run the real reference modules and demand bit-exact agreement."""
     from oracle.weights import make_lab
@@ -133,7 +133,7 @@ def test_rgb8_to_lab_oracle_anchors():
     assert int((back.int() - rgb.int()).abs().max()) <= 1
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not present (GPU box)")
+@pytest.mark.skipif(not ref_import.available(), reason="no checkout of the reference (DVC_REFERENCE_ROOT)")
 def test_contextual_loss_restatement_is_the_reference():
     """oracle.contextual_loss_forward == models/ContextualLoss.py: ContextualLoss_forward of the unmodified reference, bit for
     bit (same torch ops in the same order), on seeded feature maps of several depths."""

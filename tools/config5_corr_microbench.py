@@ -1,6 +1,6 @@
 """BASELINE.json configs[4]: the correlation-only microbench at feature maps 128^2, 256^2, 512^2 (C = 256), both
 temperatures -- this library's fused K7 against the reference's own formulation (NonlocalNet.py:477-497:
-torch.matmul -> max -> softmax(f / T) -> torch.matmul) run (a) on the same B200 through cuBLAS fp32 (TF32 off) in query-row
+torch.matmul -> max -> softmax(f / T) -> torch.matmul) run (a) on the same GPU through cuBLAS fp32 (TF32 off) in query-row
 chunks that fit HBM, and (b) on this box's CPU cores (a sub-sample of the query rows, scaled; stated in the line).
 
     python tools/config5_corr_microbench.py [--out gpurun_out/config5_r2.jsonl] [--cpu-rows 2048]

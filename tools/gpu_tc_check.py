@@ -1,4 +1,4 @@
-"""Scratch: first-light check of the tcgen05 correlation kernel against the CUDA-core one + timing."""
+"""Scratch: first-light check of the tensor-core correlation kernel against the CUDA-core one + timing."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "deep-exemplar-based-video-colorization_b200"))

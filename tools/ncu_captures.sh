@@ -1,5 +1,5 @@
 #!/bin/bash
-# `ncu --set full` captures of the kernels DESIGN.md / VERDICT.md discuss, one small CSV (raw page) per kernel under
+# `ncu --set full` captures of the tensor-core kernels, one small CSV (raw page) per kernel under
 # gpurun_out/ (the .ncu-rep files are deleted on the box: gpurun_out is capped at 64 MiB).   bash tools/ncu_captures.sh <tag>
 TAG=${1:-r2}; O=gpurun_out; mkdir -p $O
 cap() {  # name, kernel regex, launch-skip, launch-count, extra env

@@ -10,7 +10,7 @@ WANT = [
     "dram__bytes_read.sum", "dram__bytes_write.sum", "gpu__dram_throughput.avg.pct_of_peak_sustained_elapsed",
     "lts__t_bytes.sum", "lts__throughput.avg.pct_of_peak_sustained_elapsed", "l1tex__throughput.avg.pct_of_peak_sustained_elapsed",
     "l1tex__data_pipe_lsu_wavefronts_mem_shared.sum", "smsp__inst_executed_pipe_uniform.sum",
-    "sm__inst_executed_pipe_tmem.sum", "l1tex__m_xbar2l1tex_read_bytes.sum",
+    "l1tex__m_xbar2l1tex_read_bytes.sum",
     "smsp__warp_issue_stalled_long_scoreboard_per_warp_active.pct", "smsp__warp_issue_stalled_barrier_per_warp_active.pct",
     "smsp__warp_issue_stalled_wait_per_warp_active.pct", "smsp__warp_issue_stalled_sleeping_per_warp_active.pct",
 ]

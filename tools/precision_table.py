@@ -1,4 +1,4 @@
-"""Precision table for DESIGN.md: |ab - ab_fp64| of the fused frame path per engine configuration, next to the
+"""Precision table: |ab - ab_fp64| of the fused frame path per engine configuration, next to the
 reference's own fp32-vs-fp64 distance on the same inputs (tests/golden).  Run on a GPU box:
     python tools/precision_table.py > gpurun_out/precision_table.md
 """
@@ -16,12 +16,12 @@ G = lambda n: dict(np.load(os.path.join(ROOT, "tests", "golden", n + ".npz")))
 NAMES = ["small_32x48", "padbranch_40x64", "softmax_32x64", "softmax5_48x48", "default_216x384"]
 MODES = [  # label, conv math, f16 planes, kc, cluster, (unused)
     ("CUDA cores, exact fp32 (two-level sums)", dvc.MATH_FP32, 0, 1, 1, 0),
-    ("tcgen05 3xTF32, chunk 1", dvc.MATH_TF32X3, 0, 1, 2, 0),
-    ("tcgen05 3xFP16 scaled planes, chunk 1", dvc.MATH_TF32X3, 1, 1, 2, 0),
-    ("tcgen05 3xFP16 scaled planes, chunk 2", dvc.MATH_TF32X3, 1, 2, 2, 0),
-    ("tcgen05 3xFP16 scaled planes, chunk 4", dvc.MATH_TF32X3, 1, 4, 2, 0),
+    ("wgmma 3xTF32, chunk 1", dvc.MATH_TF32X3, 0, 1, 2, 0),
+    ("wgmma 3xFP16 scaled planes, chunk 1", dvc.MATH_TF32X3, 1, 1, 2, 0),
+    ("wgmma 3xFP16 scaled planes, chunk 2", dvc.MATH_TF32X3, 1, 2, 2, 0),
+    ("wgmma 3xFP16 scaled planes, chunk 4", dvc.MATH_TF32X3, 1, 4, 2, 0),
 ]
-MODES.append(("tcgen05 3xFP16 scaled planes, chunk 8", dvc.MATH_TF32X3, 1, 8, 2, 0))
+MODES.append(("wgmma 3xFP16 scaled planes, chunk 8", dvc.MATH_TF32X3, 1, 8, 2, 0))
 gs = {n: G(n) for n in NAMES}
 print("| engine | " + " | ".join(NAMES) + " | 480x864 ms/frame (one stream) |")
 print("|---|" + "---:|" * (len(NAMES) + 1))
