@@ -792,7 +792,10 @@ bool first_use_on_device(unsigned long long* mask) {
   return true;
 }
 
-static size_t screen_norm_bytes(int B, int Bphi, int NA, int NB) { return ((size_t)2 * B * NA + (size_t)2 * Bphi * NB + 8) * 4; }
+// workspace buffer 5 of the screened path: 8 cells, then the reference-side and the query-side norms (launch_corr_tc)
+static size_t screen_norm_bytes(int B, int Bphi, int NA, int NB) { return ((size_t)8 + (size_t)2 * Bphi * NB + (size_t)2 * B * NA) * 4; }
+
+const unsigned int* corr_ws_screen_cells(const CorrWorkspace* ws) { return (const unsigned int*)ws->buf[5]; }
 static size_t screen_cand_bytes(int nparts, int B, int NA) { return (size_t)nparts * B * NA * (8 + 4 * SCREEN_K); }
 
 int corr_ws_reserve(CorrWorkspace* ws, int B, int Bphi, int NA, int NB) {
@@ -875,11 +878,13 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
     const int sparts = nsplit * QUADS;
     if (ws_get(ws, 5, screen_norm_bytes(p.B, p.Bphi, p.NA, p.NB), &norms) || ws_get(ws, 6, screen_cand_bytes(sparts, p.B, p.NA), &cand))
       return fail("workspace allocation failed");
-    float* nd_a = (float*)norms;
-    float* nh_a = nd_a + rows;
-    float* nd_b = nh_a + rows;
+    // cells [8] | nd_b [rphi] | nh_b [rphi] | nd_a [rows] | nh_a [rows]: the reference side must not move with the query
+    // row count, because a cached reference side is read again by calls with fewer query rows
+    unsigned int* cells = (unsigned int*)norms;  // [0,1]: query side (unused maxima), [2,3]: reference side, [4..7]: padding
+    float* nd_b = (float*)(cells + 8);
     float* nh_b = nd_b + rphi;
-    unsigned int* cells = (unsigned int*)(nh_b + rphi);  // [0,1]: query side (unused maxima), [2,3]: reference side
+    float* nd_a = nh_b + rphi;
+    float* nh_a = nd_a + rows;
     const bool phi_cached = phi_version >= 0 && ws->phi_src == p.phi && ws->phi_version == phi_version && ws->phi_fmt == 3 &&
                             ws->phi_elems == ephi;
     if (cudaMemsetAsync(cells, 0, (phi_cached ? 2 : 4) * sizeof(unsigned int), s) != cudaSuccess) return fail("cudaMemsetAsync failed");

@@ -21,6 +21,9 @@ struct CorrWorkspace {
 // reserve for B x NA query rows against Bphi x NB reference rows (any math mode, any split count); 0 on success
 int corr_ws_reserve(CorrWorkspace* ws, int B, int Bphi, int NA, int NB);
 void corr_ws_free(CorrWorkspace* ws);
+// the 4 max cells of the screened path (float bits): [0, 1] query side, [2, 3] reference side (||dropped part||, ||hi
+// part|| maxima); nullptr while the workspace is unallocated.  Debug / tests.
+const unsigned int* corr_ws_screen_cells(const CorrWorkspace* ws);
 // math = DVC_MATH_TF32X3 / BF16X3 / FP16X3.  Returns 0 on success, non-zero with *err set otherwise.
 // cluster: 2 = 2-CTA clusters on adjacent query-row tiles sharing the multicast reference tile, 1 = single CTAs
 // phi_version >= 0: the caller guarantees that p.phi's contents change only together with phi_version (the planes of

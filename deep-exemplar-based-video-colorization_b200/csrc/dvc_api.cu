@@ -1167,6 +1167,12 @@ extern "C" int dvc_debug_get_buffer(dvc_ctx* c, const char* name, void** dev_ptr
   if (!c || !name || !dev_ptr || !bytes) return DVC_ERR_ARG;
   if (!strcmp(name, "ex.phi")) { *dev_ptr = c->ex_phi; *bytes = (int64_t)c->ex_N * 256 * 4; return DVC_OK; }
   if (!strcmp(name, "ex.V")) { *dev_ptr = c->ex_V; *bytes = (int64_t)c->ex_N * 16; return DVC_OK; }
+  if (!strcmp(name, "corr.screen_cells")) {
+    const unsigned int* cells = corr_ws_screen_cells(&c->corr_ws);
+    if (!cells) return fail(c, DVC_ERR_STATE, "corr.screen_cells: no screened correlation has run");
+    *dev_ptr = (void*)cells, *bytes = 16;
+    return DVC_OK;
+  }
   auto it = c->bufs.find(name);
   if (it == c->bufs.end()) return fail(c, DVC_ERR_ARG, std::string("no such buffer: ") + name);
   *dev_ptr = it->second.p;

@@ -215,7 +215,8 @@ int dvc_conv_profile(dvc_ctx* ctx, int variant, int reset, double* total_ms, dou
  *   dvc_debug_set_flag: "two_level" (default 1) selects per-tap two-level fp32 accumulation in the
  *   CUDA-core convolution (shorter rounding chain; 0 = plain sequential accumulation, faster).
  *   dvc_debug_get_buffer: device pointer / size of a named internal workspace (padded NHWC activations
- *   carry their [B,H,W,C,P] signature in sig5) so tests can check intermediate stages. */
+ *   carry their [B,H,W,C,P] signature in sig5) so tests can check intermediate stages.  "corr.screen_cells" is the
+ *   screened T -> 0 correlation's 4 maxima (float bits): query-side ||dropped||, ||hi||, then reference-side. */
 int dvc_debug_set_flag(dvc_ctx* ctx, const char* name, int value);
 int dvc_debug_get_buffer(dvc_ctx* ctx, const char* name, void** dev_ptr, int64_t* bytes, int* sig5);
 /*   dvc_debug_conv2d: ONE convolution layer (the weights `name` of network `net`, already set with dvc_set_weight) on a
