@@ -445,8 +445,9 @@ __global__ void __launch_bounds__(NTHREADS, 1)
           }
         }
         if (p.stats && uniform_img) {
-          // the warp's 16 pixel rows of these two channels: butterfly over the 8 lanes that share qd (fixed order, so the
-          // statistics -- and with them the whole forward -- are run-to-run deterministic)
+          // the warp's 16 pixel rows of these two channels: butterfly over the 8 lanes that share qd (fixed order within
+          // the tile; the tiles' double atomics below land in completion order, and the per-pixel double squares of tiles
+          // that straddle an image boundary make the last bits of those sums depend on it)
 #pragma unroll
           for (int off = 4; off <= 16; off <<= 1) {
 #pragma unroll

@@ -1370,8 +1370,11 @@ extern "C" int dvc_debug_conv2d(dvc_ctx* c, int net, const char* name, const flo
   DVC_TRY(need_conv(c, net, name, &w));
   DVC_TRY(stats_begin(c, s));
   const bool tcm = tc_mode(c) && w->wt_hi, f16 = tcm && c->tc_f16;
+  // the first layers (no tensor-core weights) store device-scaled planes in the fp16 engine's mode, like vgg_trunk
+  const bool first_dyn = tc_mode(c) && c->tc_f16 && !w->wt_hi;
   if ((upconv || fuse_tail) && !tcm) return fail(c, DVC_ERR_STATE, "debug_conv2d: phase / fused-tail layers need the tensor-core engine");
-  if (out_planes && !f16) return fail(c, DVC_ERR_STATE, "debug_conv2d: device-scaled output planes need the fp16 engine");
+  if (out_planes && !f16 && !first_dyn) return fail(c, DVC_ERR_STATE, "debug_conv2d: device-scaled output planes need the fp16 engine");
+  if (in_bound < 0.f && tcm) return fail(c, DVC_ERR_ARG, "debug_conv2d: a measured input bound (in_bound < 0) is for the first layers");
   Act x0, xp, yo, addA;
   DVC_TRY(get_act(c, "dbg.x0", B, H, W, w->cin_pad, 0, &x0, s));
   launch_nchw_to_act(x, w->cin, x0.d, nullptr, B, H, W, w->cin_pad, 0, PAD_ZERO, 0, s);
@@ -1381,6 +1384,11 @@ extern "C" int dvc_debug_conv2d(dvc_ctx* c, int net, const char* name, const flo
   XfOpt xo;
   xo.pad_mode = pad_mode ? PAD_REFLECT : PAD_ZERO;
   DVC_TRY(run_xform(c, x0, xp, xo, s));
+  if (in_bound < 0.f) {  // max |x| measured on the device (the first layer of a trunk: vgg_trunk, colorvid)
+    DVC_TRY(cell_alloc(c, &xp.cell, s));
+    launch_amax(xp.d, xp.elems(), xp.cell, s);
+    DVC_TRY(check_launch(c, "amax"));
+  }
   const int Ho = upconv ? 2 * H : (H + stride - 1) / stride, Wo = upconv ? 2 * W : (W + stride - 1) / stride;
   ConvOpt o;
   o.dil = dil, o.stride = stride, o.act = act, o.slope = slope;

@@ -418,7 +418,10 @@ class Context:
     def debug_conv2d(self, net, name, x, cout, dil=1, stride=1, act=0, slope=0.0, reflect=False, upconv=False,
                      fuse_tail=False, in_bound=None, out_planes=False, add=None, want_stats=False):
         """One convolution layer (weights `name` of `net`) on a CUDA NCHW tensor through the engine the layer programs
-        use (include/dvc.h: dvc_debug_conv2d).  Returns y or (y, stats [B,cout,2] float64)."""
+        use (include/dvc.h: dvc_debug_conv2d).  Returns y or (y, stats [B,cout,2] float64).
+
+        in_bound: a bound of max |x| (default: x.abs().max()), or a negative value for the first layers (Cin <= 8), whose
+        max |x| is then measured on the device; out_planes=True on a first layer needs that measured bound."""
         x = _dev_f32(x, "debug_conv2d input")
         B, _, H, W = x.shape
         Ho, Wo = (2 * H, 2 * W) if upconv else ((H + stride - 1) // stride, (W + stride - 1) // stride)

@@ -224,8 +224,10 @@ int dvc_debug_get_buffer(dvc_ctx* ctx, const char* name, void** dev_ptr, int64_t
  *   current dvc_set_math and debug flags ("tc_force_bn" = 64 / 128 / 256 pins the channel tile) -- the per-layer parity
  *   tests compare it with an fp64 F.conv2d (nn.Conv2d at NonlocalNet.py:235-255,364-423, ColorVidNet.py:96-143).
  *   pad_mode 0 = zero padding, 1 = ReflectionPad2d; act 0 none / 1 ReLU / 2 LeakyReLU(slope); in_bound >= max |x|
- *   (fixes the exact power-of-two scale of the fp16 operand planes); out_planes = 1 stores the result as fp16 hi/lo
- *   planes with the device-derived exponent and reads it back; upconv = 1: Upsample(2, nearest) + Conv2d(3x3) as four
+ *   (fixes the exact power-of-two scale of the fp16 operand planes), or in_bound < 0 for the first layers (Cin <= 8, no
+ *   tensor-core weights): max |x| is measured on the device, as the VGG and ColorVidNet layer programs do; out_planes = 1
+ *   stores the result as fp16 hi/lo planes with the device-derived exponent and reads it back (the first layers need
+ *   in_bound < 0 for that); upconv = 1: Upsample(2, nearest) + Conv2d(3x3) as four
  *   phase convolutions (y is [B][Cout][2H][2W]); fuse_tail = 1: conv10_2 + LeakyReLU + conv10_ab + tanh*128 (y is
  *   [B][2][H][W]); add: optional device NCHW addend of the output's shape; stats_out: optional device [B][Cout][2]
  *   doubles receiving (sum, sum of squares) over positions. */

@@ -78,15 +78,17 @@ LAYERS = [
 _REF = {}  # the CPU fp64 / fp32 references are shared by the engine / tile variants of a layer
 
 
-def reference(sds, net, name, cin, cout, H, W, B, seed, nonneg, with_add, fuse_tail, kw):
+def reference(sds, net, name, cin, cout, H, W, B, seed, nonneg, with_add, fuse_tail, kw, sd=None):
     key = (net, name, H, W, B, seed, nonneg, with_add, fuse_tail, tuple(sorted(kw.items())))
     if key not in _REF:
-        sd = sds[NETKEY[net]]
+        sd = sds[NETKEY[net]] if sd is None else sd
         assert tuple(sd[name + ".weight"].shape[:2]) == (cout, cin), (name, sd[name + ".weight"].shape)
         x = make_input(1234 + seed, B, cin, H, W, nonneg)
         add = None
-        if with_add:
-            add = torch.randn(B, cout, 2 * H, 2 * W, generator=torch.Generator().manual_seed(99 + seed)) * 3
+        if with_add:  # an addend of the output's shape
+            st = kw.get("stride", 1)
+            Ho, Wo = (2 * H, 2 * W) if kw.get("upconv") else ((H + st - 1) // st, (W + st - 1) // st)
+            add = torch.randn(B, cout, Ho, Wo, generator=torch.Generator().manual_seed(99 + seed)) * 3
         with torch.no_grad():
             y64 = ref_conv(sd, name, x, add=add, **kw)
             y32 = ref_conv(sd, name, x, add=add, dtype=torch.float32, **kw)
@@ -97,15 +99,17 @@ def reference(sds, net, name, cin, cout, H, W, B, seed, nonneg, with_add, fuse_t
     return _REF[key]
 
 
-def run_layer(ctx, sds, net, name, cin, cout, H, W, B=1, seed=0, out_planes=False, **kw):
+def run_layer(ctx, sds, net, name, cin, cout, H, W, B=1, seed=0, out_planes=False, sd=None, in_bound=None, **kw):
+    """One layer through dvc_debug_conv2d against fp64.  sd: the layer's own state dict (synthetic layers loaded under
+    test-only names) instead of the network's.  Returns (max error, reference fp32 floor), both relative to max |y64|."""
     kw = dict(kw)
     nonneg, with_add, want_stats = kw.pop("nonneg", False), kw.pop("with_add", False), kw.pop("want_stats", False)
     fuse_tail = kw.pop("fuse_tail", False)
-    x, add, y64, y32 = reference(sds, net, name, cin, cout, H, W, B, seed, nonneg, with_add, fuse_tail, kw)
+    x, add, y64, y32 = reference(sds, net, name, cin, cout, H, W, B, seed, nonneg, with_add, fuse_tail, kw, sd)
     res = ctx.debug_conv2d(net, name, x.cuda(), cout, dil=kw.get("dil", 1), stride=kw.get("stride", 1), act=kw.get("act", 0),
                            slope=kw.get("slope", 0.0), reflect=kw.get("reflect", False), upconv=kw.get("upconv", False),
                            fuse_tail=fuse_tail, out_planes=out_planes, add=add.cuda() if add is not None else None,
-                           want_stats=want_stats)
+                           want_stats=want_stats, in_bound=in_bound)
     y, st = res if want_stats else (res, None)
     y = y.cpu().double()
     scale = y64.abs().max().item()

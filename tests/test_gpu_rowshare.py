@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from conftest import load_golden
-from test_gpu_conv_layers import BENCH, LAYERS, run_layer
+from test_gpu_conv_layers import BENCH, COLOR, LAYERS, run_layer
 
 pytestmark = pytest.mark.gpu
 MODES = [int(m) for m in os.environ.get("DVC_TEST_ROWSHARE", "").split(",") if m]
@@ -37,6 +37,37 @@ def test_layer_rowshare_vs_fp64(ctx, sds, rowshare, layer, force_bn, cluster):
     ctx.debug_flag("tc_force_bn", force_bn)
     ctx.debug_flag("tc_cluster", cluster)
     err, floor = run_layer(ctx, sds, net, name, cin, cout, H, W, **kw)
+    assert err <= 4e-6, (layer[0], force_bn, cluster, rowshare, err, floor)
+
+
+# dilation 3 and 4 shift the taps of a row by 3 / 6 and 4 / 8 rows of the shared tile (the nets only use 1 and 2);
+# synthetic layers of test_gpu_conv_edges.py, (cin, cout, H, W, B, kwargs)
+DILATED = [
+    ("d3_c64_o72", 64, 72, 7, 17, 1, dict(dil=3, act=1)),
+    ("d4_c256_o200_b2_stats", 256, 200, 5, 13, 2, dict(dil=4, want_stats=True)),
+    ("d3_c64_o320_lrelu", 64, 320, 11, 29, 1, dict(dil=3, act=2, slope=0.2)),
+    ("d4_c256_o264_b3_relu", 256, 264, 3, 3, 3, dict(dil=4, act=1)),
+    ("d2_c64_o40_reflect_w3", 64, 40, 5, 3, 3, dict(dil=2, reflect=True, want_stats=True)),
+]
+
+
+@pytest.mark.parametrize("cluster", [2, 1])
+@pytest.mark.parametrize("force_bn", [0, 256, 128, 64])
+@pytest.mark.parametrize("layer", DILATED, ids=lambda l: l[0])
+def test_dilated_rowshare_vs_fp64(request, ctx, sds, rowshare, layer, force_bn, cluster):
+    from test_gpu_conv_edges import cout_pad_tc, load_synthetic
+
+    if rowshare == 2:  # strict: a fix of the base-offset variant must turn these into passes
+        request.node.add_marker(pytest.mark.xfail(strict=True, reason="the descriptor base-offset variant (tc_rowshare = 2, off "
+                                                  "by default) computes dilated layers wrongly on sm_90a (error ~0.9 of max |y|)"))
+
+    _, cin, cout, H, W, B, kw = layer
+    if force_bn and cout_pad_tc(cout) % force_bn:
+        pytest.skip("the channel tile does not divide the padded Cout")
+    name, sd = load_synthetic(ctx, cin, cout)
+    ctx.debug_flag("tc_force_bn", force_bn)
+    ctx.debug_flag("tc_cluster", cluster)
+    err, floor = run_layer(ctx, sds, COLOR, name, cin, cout, H, W, B=B, sd=sd, **kw)
     assert err <= 4e-6, (layer[0], force_bn, cluster, rowshare, err, floor)
 
 
