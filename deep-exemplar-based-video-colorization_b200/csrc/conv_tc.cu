@@ -17,12 +17,13 @@
 //   warps 4..11  two consumer warpgroups.  Tile 128 px x 64 / 128 channels: each warpgroup owns 64 pixels; tile 64 px x
 //                256 channels: each owns 128 channels.  Per k-block 4 k-steps x 3 wgmma (the two cross terms of the whole
 //                k-block first, hi.hi last) into fp32 registers; every chunk (kc k-blocks) that partial sum is added to
-//                fp32 register totals with round-to-nearest adds (the tensor-core accumulation truncates); then + bias,
+//                fp32 register totals with round-to-nearest adds (the tensor-core accumulation truncates) while the next
+//                chunk's wgmma run into a second set of accumulator registers; then + bias,
 //                + skip addend, activation, InstanceNorm statistics (shuffle reduction over the warp's pixels -> one
 //                double atomic per channel and tile), measured max |y|, masked store of the interior pixels as fp32 /
 //                tf32 planes / fp16 planes -- or the fused 1x1 + tanh tail of ColorVidNet instead of a store.
-// The channel tile is capped by the register file: partial sum + total of a 128 x 128 (or 64 x 256) tile take all of
-// the consumers' registers.
+// The channel tile is capped by the register file: two partial sums + total of a 128 x 128 (or 64 x 256) tile take 192
+// of the consumers' registers.
 // Replaces nn.Conv2d (+ReLU/LeakyReLU/skip add) at NonlocalNet.py:235-255,364-423 and ColorVidNet.py:96-143.
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -83,19 +84,6 @@ __device__ __forceinline__ float tf32_rna(float x) {
   uint32_t u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
   return __uint_as_float(u);
-}
-
-template <int CL>
-__device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
-  __syncwarp();
-  if (lane == 0) {
-    if (CL == 1) {
-      tc::mbar_arrive(bar);
-    } else {
-#pragma unroll
-      for (int r = 0; r < CL; ++r) tc::mbar_arrive_cluster(bar, (uint32_t)r);
-    }
-  }
 }
 
 // CL = 2: the kernel runs as 2-CTA clusters on adjacent pixel tiles of the same channel tile; each CTA loads its own
@@ -258,97 +246,42 @@ __global__ void __launch_bounds__(NTHREADS, 1)
         if (ctid == 0 && blockIdx.x == 0) p.dyn.cell_out->e = e_out;
       }
     }
-    int stage = 0, as = 0, bs = 0;
-    uint32_t phase = 0, aph = 0, bph = 0;
-    float acc[R], tot[R];
-    for (int work = item0; work < total_work; work += item_stride) {
-      const int sp = work / total_items, item = work - sp * total_items;
+    float acc0[R], acc1[R], tot[R];
+    // workspace layout [tile][register][consumer thread]: coalesced hand-over of the running totals
+    auto tile_of = [&](int w) {
+      const int item = w % total_items, mg = item / n_tiles;
+      return (mg * CL + crank) * n_tiles + (item - mg * n_tiles);
+    };
+    // Totals of work item w before its first chunk: -0 (the identity of the round-to-nearest adds, so the first chunk
+    // lands in them bit for bit), or what split sp - 1 left in the workspace
+    auto start_item = [&](int w) {
+      const int sp = w / total_items;
+      if (sp == 0) {
+#pragma unroll
+        for (int j = 0; j < R; ++j) tot[j] = -0.f;
+        return;
+      }
+      const int tile_id = tile_of(w);
+      if (ctid == 0) {
+        const int want = p.epoch * 16 + sp;
+        int got;
+        do {
+          asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(got) : "l"(p.flags + tile_id) : "memory");
+        } while (got != want);
+      }
+      epi_sync();
+      const float* wsp = p.ws + (size_t)tile_id * BN * BMT + ctid;
+#pragma unroll
+      for (int j = 0; j < R; ++j) tot[j] = __ldcg(wsp + (size_t)j * CONSUMERS);
+    };
+    // Epilogue of work item w on its totals
+    auto finish_item = [&](int w) {
+      const int sp = w / total_items, item = w - sp * total_items;
       const int mg = item / n_tiles, nt = item - mg * n_tiles;
       const int m0 = px0 + (mg * CL + crank) * BMT, n0 = nt * BN;
-      const int tile_id = (mg * CL + crank) * n_tiles + nt;
-      // workspace layout [tile][register][consumer thread]: coalesced hand-over of the running totals
-      float* wsp = p.ws + (size_t)tile_id * BN * BMT + ctid;
-      if (sp > 0) {
-        if (ctid == 0) {
-          const int want = p.epoch * 16 + sp;
-          int got;
-          do {
-            asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(got) : "l"(p.flags + tile_id) : "memory");
-          } while (got != want);
-        }
-        epi_sync();
-#pragma unroll
-        for (int j = 0; j < R; ++j) tot[j] = __ldcg(wsp + (size_t)j * CONSUMERS);
-      }
-      const int ch_lo = nchunks * sp / S, ch_hi = nchunks * (sp + 1) / S;
-      for (int ch = ch_lo; ch < ch_hi; ++ch) {
-        const int k_end = min((ch + 1) * kc, nk);
-        for (int k = ch * kc; k < k_end; ++k) {
-          uint32_t sa, sb;
-          uint64_t bo = 0;
-          int tx = 0, ntx = 1;
-          if constexpr (RS) {
-            ntx = p.rs_ntx;
-            const int g = k / ntx, ty = g / kbs;
-            tx = k - g * ntx;
-            if (tx == 0) tc::mbar_wait(&full[as], aph);  // the activation tile of this (tap row, k-block)
-            tc::mbar_wait(&full[RC::A_STAGES + bs], bph);
-            // the tap's rows start (tap_off[tap] - tap_off[first tap of the row]) rows into the shared tile
-            // (p.dbg & 1: TIMING EXPERIMENT ONLY, wrong results -- every tap reads the tile at its aligned start)
-            const int shift = (p.dbg & 1) ? 0 : p.tap_off[ty * ntx + tx] - p.tap_off[ty * ntx];
-            sa = tc::smem_u32(smem + as * RC::A_STAGE) + (uint32_t)(ro + shift) * 128u;
-            sb = tc::smem_u32(smem + RC::A_STAGES * RC::A_STAGE + bs * RC::B_STAGE) + (uint32_t)co * 128u;
-            bo = p.rs_base_offset ? ((uint64_t)(shift & 7) << 49) : 0ull;
-          } else {
-            tc::mbar_wait(&full[stage], phase);
-            sa = tc::smem_u32(smem + stage * C::STAGE_BYTES) + (uint32_t)ro * KBY;
-            sb = tc::smem_u32(smem + stage * C::STAGE_BYTES + 2 * A_BYTES) + (uint32_t)co * KBY;
-          }
-          constexpr uint32_t A_PLANE = RS ? RC::A_TILE : A_BYTES, B_PLANE = RS ? RC::B_TILE : C::B_BYTES;
-          auto mkdesc = [](uint32_t a) { return KBY == 128 ? tc::wg_desc_k128(a) : tc::wg_desc_k64(a); };
-          const uint64_t dXh = mkdesc(sa) | bo, dXl = mkdesc(sa + A_PLANE) | bo;
-          const uint64_t dWh = mkdesc(sb), dWl = mkdesc(sb + B_PLANE);
-          tc::wg_fence_regs(acc);
-          tc::wg_fence();
-          // Every accumulation truncates the accumulator at ITS current magnitude, so the two small cross terms of the
-          // whole k-block go first (while a fresh accumulator is still ~2^-11 of its final size, their truncations are
-          // negligible) and the dominant hi*hi terms last: 4 instead of 12 full-size truncations per k-block.
-#pragma unroll
-          for (int kk = 0; kk < KBY / 32; ++kk) {
-            const uint64_t adv = (uint64_t)(kk * 2);
-            tc::wgmma_fmt<FMT>(acc, dXl + adv, dWh + adv, (k > ch * kc || kk) ? 1u : 0u);
-            tc::wgmma_fmt<FMT>(acc, dXh + adv, dWl + adv, 1u);
-          }
-#pragma unroll
-          for (int kk = 0; kk < KBY / 32; ++kk) {
-            const uint64_t adv = (uint64_t)(kk * 2);
-            tc::wgmma_fmt<FMT>(acc, dXh + adv, dWh + adv, 1u);
-          }
-          tc::wg_commit();
-          tc::wg_wait<0>();
-          if constexpr (RS) {
-            release_stage<CL>(&empty[RC::A_STAGES + bs], lane);
-            if (++bs == RC::B_STAGES) bs = 0, bph ^= 1;
-            if (tx == ntx - 1) {
-              release_stage<CL>(&empty[as], lane);
-              if (++as == RC::A_STAGES) as = 0, aph ^= 1;
-            }
-          } else {
-            release_stage<CL>(&empty[stage], lane);
-            if (++stage == C::STAGES) stage = 0, phase ^= 1;
-          }
-        }
-        tc::wg_fence_regs(acc);
-        if (ch == 0) {  // first chunk of the tile (always in split 0)
-#pragma unroll
-          for (int j = 0; j < R; ++j) tot[j] = acc[j];
-        } else {
-#pragma unroll
-          for (int j = 0; j < R; ++j) tot[j] += acc[j];
-        }
-      }
-
+      const int tile_id = tile_of(w);
       if (sp < S - 1) {  // hand the running totals to the next split of this tile
+        float* wsp = p.ws + (size_t)tile_id * BN * BMT + ctid;
 #pragma unroll
         for (int j = 0; j < R; ++j) __stcg(wsp + (size_t)j * CONSUMERS, tot[j]);
         __threadfence();
@@ -357,7 +290,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
           const int v = p.epoch * 16 + sp + 1;
           asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p.flags + tile_id), "r"(v) : "memory");
         }
-        continue;
+        return;
       }
 
       // ---- bias, skip addend, activation, statistics, masked store ----
@@ -495,6 +428,110 @@ __global__ void __launch_bounds__(NTHREADS, 1)
         }
         epi_sync();
       }
+    };
+
+    int stage = 0, as = 0, bs = 0;  // ring positions of the next k-block
+    uint32_t phase = 0, aph = 0, bph = 0;
+    int prev_stage = -1, prev_a = -1;  // ring stages the k-block in flight frees when retired (-1: none)
+    auto retire_prev = [&]() {
+      tc::release_stage<CL>(&empty[prev_stage], lane);
+      if (RS && prev_a >= 0) tc::release_stage<CL>(&empty[prev_a], lane);
+    };
+    // Issue k-block k into the accumulator set `a` (FIRST: the first of its chunk, which overwrites `a`), then retire
+    // the k-block issued before it
+    auto kblock = [&](float (&a)[R], int k, bool first) {
+      uint32_t sa, sb;
+      uint64_t bo = 0;
+      int tx = 0, ntx = 1;
+      if constexpr (RS) {
+        ntx = p.rs_ntx;
+        const int g = k / ntx, ty = g / kbs;
+        tx = k - g * ntx;
+        if (tx == 0) tc::mbar_wait(&full[as], aph);  // the activation tile of this (tap row, k-block)
+        tc::mbar_wait(&full[RC::A_STAGES + bs], bph);
+        // the tap's rows start (tap_off[tap] - tap_off[first tap of the row]) rows into the shared tile
+        // (p.dbg & 1: TIMING EXPERIMENT ONLY, wrong results -- every tap reads the tile at its aligned start)
+        const int shift = (p.dbg & 1) ? 0 : p.tap_off[ty * ntx + tx] - p.tap_off[ty * ntx];
+        sa = tc::smem_u32(smem + as * RC::A_STAGE) + (uint32_t)(ro + shift) * 128u;
+        sb = tc::smem_u32(smem + RC::A_STAGES * RC::A_STAGE + bs * RC::B_STAGE) + (uint32_t)co * 128u;
+        bo = p.rs_base_offset ? ((uint64_t)(shift & 7) << 49) : 0ull;
+      } else {
+        tc::mbar_wait(&full[stage], phase);
+        sa = tc::smem_u32(smem + stage * C::STAGE_BYTES) + (uint32_t)ro * KBY;
+        sb = tc::smem_u32(smem + stage * C::STAGE_BYTES + 2 * A_BYTES) + (uint32_t)co * KBY;
+      }
+      constexpr uint32_t A_PLANE = RS ? RC::A_TILE : A_BYTES, B_PLANE = RS ? RC::B_TILE : C::B_BYTES;
+      auto mkdesc = [](uint32_t x) { return KBY == 128 ? tc::wg_desc_k128(x) : tc::wg_desc_k64(x); };
+      const uint64_t dXh = mkdesc(sa) | bo, dXl = mkdesc(sa + A_PLANE) | bo;
+      const uint64_t dWh = mkdesc(sb), dWl = mkdesc(sb + B_PLANE);
+      tc::wg_fence_regs(a);
+      tc::wg_fence();
+      // Every accumulation truncates the accumulator at ITS current magnitude, so the two small cross terms of the
+      // whole k-block go first (while a fresh accumulator is still ~2^-11 of its final size, their truncations are
+      // negligible) and the dominant hi*hi terms last: 4 instead of 12 full-size truncations per k-block.
+#pragma unroll
+      for (int kk = 0; kk < KBY / 32; ++kk) {
+        const uint64_t adv = (uint64_t)(kk * 2);
+        tc::wgmma_fmt<FMT>(a, dXl + adv, dWh + adv, (first && kk == 0) ? 0u : 1u);
+        tc::wgmma_fmt<FMT>(a, dXh + adv, dWl + adv, 1u);
+      }
+#pragma unroll
+      for (int kk = 0; kk < KBY / 32; ++kk) {
+        const uint64_t adv = (uint64_t)(kk * 2);
+        tc::wgmma_fmt<FMT>(a, dXh + adv, dWh + adv, 1u);
+      }
+      tc::wg_commit();
+      tc::wg_wait<1>();  // unconditional (a no-op without an older group), so ptxas sees every older group retired
+      if (prev_stage >= 0) retire_prev();
+      if constexpr (RS) {
+        prev_stage = RC::A_STAGES + bs, prev_a = tx == ntx - 1 ? as : -1;
+        if (++bs == RC::B_STAGES) bs = 0, bph ^= 1;
+        if (tx == ntx - 1 && ++as == RC::A_STAGES) as = 0, aph ^= 1;
+      } else {
+        prev_stage = stage;
+        if (++stage == C::STAGES) stage = 0, phase ^= 1;
+      }
+    };
+    // Chunk ch into set `a`; once its first k-block is issued, the previous chunk (set `o`, PROMOTE) has been retired
+    // by kblock's wgmma.wait_group 1 and is added to the totals while `a` is in flight
+    auto chunk = [&](float (&a)[R], float (&o)[R], int ch, bool promote) {
+      const int k0 = ch * kc, k_end = min(k0 + kc, nk);
+      kblock(a, k0, true);
+      if (promote) {
+        tc::wg_fence_regs(o);
+#pragma unroll
+        for (int j = 0; j < R; ++j) tot[j] += o[j];
+      }
+      for (int k = k0 + 1; k < k_end; ++k) kblock(a, k, false);
+    };
+    // the last chunk of a work item
+    auto drain = [&](float (&a)[R]) {
+      tc::wg_wait<0>();
+      tc::wg_fence_regs(a);
+      retire_prev();
+      prev_stage = -1;
+#pragma unroll
+      for (int j = 0; j < R; ++j) tot[j] += a[j];
+    };
+    for (int work = item0; work < total_work; work += item_stride) {
+      const int sp = work / total_items;
+      start_item(work);
+      // consecutive chunks alternate between the two accumulator sets
+      const int ch_lo = nchunks * sp / S, ch_hi = nchunks * (sp + 1) / S;
+      for (int ch = ch_lo;;) {
+        chunk(acc0, acc1, ch, ch > ch_lo);
+        if (++ch == ch_hi) {
+          drain(acc0);
+          break;
+        }
+        chunk(acc1, acc0, ch, true);
+        if (++ch == ch_hi) {
+          drain(acc1);
+          break;
+        }
+      }
+
+      finish_item(work);
     }
     if (F16 && p.dyn.cell_out) warp_amax_commit(amax, p.dyn.cell_out);
   }

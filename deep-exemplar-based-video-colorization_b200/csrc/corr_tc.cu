@@ -85,21 +85,6 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
                "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(tc::smem_u32(bar))
                : "memory");
 }
-// a consumer warp hands a ring stage back: in a cluster the stage of EVERY CTA must be free before a producer
-// multicasts into it, so each consumer warp arrives on the "empty" barrier of both CTAs
-template <int CL>
-__device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
-  __syncwarp();
-  if (lane == 0) {
-    if (CL == 1) {
-      tc::mbar_arrive(bar);
-    } else {
-#pragma unroll
-      for (int r = 0; r < CL; ++r) tc::mbar_arrive_cluster(bar, (uint32_t)r);
-    }
-  }
-}
-
 // per (split part, row) partial statistics.  Softmax: running max m, sum s of exp weights, weighted colour sums a*.
 // Argmax: max m, lowest column idx attaining it, s = NUMBER of columns whose score equals m bit for bit and a* = the sum
 // of their V rows -- the reference's fp32 softmax(f / 1e-10) averages the V rows of bit-equal maxima (duplicated
@@ -327,14 +312,14 @@ __global__ void __launch_bounds__(NTHREADS, 1)
         tc::wg_commit();
         if (prev >= 0) {  // the previous k-block's MMAs have read their stage: hand it back
           tc::wg_wait<1>();
-          release_stage<CL>(&empty[prev], lane);
+          tc::release_stage<CL>(&empty[prev], lane);
         }
         prev = stage;
         if (++stage == STAGES) stage = 0, phase ^= 1;
       }
       tc::wg_wait<0>();
       tc::wg_fence_regs(acc);
-      release_stage<CL>(&empty[prev], lane);
+      tc::release_stage<CL>(&empty[prev], lane);
 
       const int buf = t & 1;
       if (SOFTMAX) tc::mbar_wait(&vfull[buf], (t >> 1) & 1);
@@ -552,14 +537,14 @@ __global__ void __launch_bounds__(NTHREADS, 1)
         tc::wg_commit();
         if (prev >= 0) {
           tc::wg_wait<1>();
-          release_stage<CL>(&empty[prev], lane);
+          tc::release_stage<CL>(&empty[prev], lane);
         }
         prev = stage;
         if (++stage == STAGES) stage = 0, phase ^= 1;
       }
       tc::wg_wait<0>();
       tc::wg_fence_regs(acc);
-      release_stage<CL>(&empty[prev], lane);
+      tc::release_stage<CL>(&empty[prev], lane);
 
       const int colbase = (t0 + t) * BN;
 #pragma unroll

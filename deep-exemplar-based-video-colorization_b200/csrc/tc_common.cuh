@@ -35,16 +35,27 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// arrive on the mbarrier at `bar`'s offset in CTA `rank` of the cluster (may be this CTA)
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(rank)
-      : "memory");
+// A consumer warp hands a ring stage back to the producer.  In a cluster of CL CTAs the stage of EVERY CTA must be free
+// before a producer multicasts into it, so lane r arrives on the "empty" barrier at `bar`'s offset in CTA r (lanes
+// 0..CL-1 in one instruction).  The arrive has the default .release.cta semantics, which ptxas emits without a
+// GPU-scope fence (a .release.cluster arrive costs a MEMBAR.ALL.GPU per call).  That is enough ONLY because every read
+// of the stage is a wgmma that wgmma.wait_group has retired before this call: no generic-proxy access to the stage is
+// left to order against the producer's next TMA write into it.
+template <int CL>
+__device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
+  __syncwarp();
+  if (CL == 1) {
+    if (lane == 0) mbar_arrive(bar);
+  } else if (lane < CL) {
+    asm volatile(
+        "{\n\t"
+        ".reg .b32 ra;\n\t"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
+        "}\n" ::"r"(smem_u32(bar)),
+        "r"(lane)
+        : "memory");
+  }
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t done = 0;
