@@ -145,6 +145,7 @@ struct dvc_ctx {
   int tc_tail = 0;        // tensor-core convolutions: 1 = 128-channel tiles for the partial last round of 256-channel
                           // launches (-1.3 % on one stream, +1.6 % in the two-stream clip pipeline: off by default)
   int tc_f16 = 1;         // tensor-core convolutions: fp16 hi/lo planes for layers with provably bounded inputs
+  int keep_stages = 0;    // tests: WarpNet's residual blocks and projection write buffers of their own (see warp_side)
   std::unordered_map<std::string, float> vec_absmax[3];  // max |scale| of the *_ss vectors
   int tc_cluster = 2;     // tensor-core convolutions: 2 = 2-CTA clusters sharing the multicast weight tile, 1 = single CTAs
   int tc_kc = 1;          // tensor-core convolutions: k-blocks per accumulator chunk (see conv_tc.cu)
@@ -677,6 +678,7 @@ static int run_xform(dvc_ctx* c, const Act& src, Act& dst, const XfOpt& o, cudaS
 static int run_pixnorm(dvc_ctx* c, const Act& src, float* dst, float* dst_lo, int dP, int pad_mode, const double* stats,
                        double count, cudaStream_t s, void* h16 = nullptr, void* l16 = nullptr, int e16 = 0) {
   if (src.C != 128 && src.C != 256 && src.C != 512) return fail(c, DVC_ERR_SHAPE, "pixnorm: channel count");
+  if (pad_mode == PAD_REFLECT && (dP >= src.H || dP >= src.W)) return fail(c, DVC_ERR_SHAPE, "pixnorm: reflect pad too wide");
   PixNormParams p{};
   p.src = src.d, p.src_lo = src.lo, p.sH = src.H, p.sW = src.W, p.sP = src.P, p.sC = src.C;
   if (src.h16 && !src.d) {
@@ -823,13 +825,26 @@ static int warp_side(dvc_ctx* c, const std::string& tag, const Act n[4], const c
     DVC_TRY(run_xform(c, raw2, cat, x2, s));
   }
 
-  // three residual blocks (NonlocalNet.py:341-352), ping-pong between two padded buffers
-  Act xa = cat, xb, raw, mid;
-  DVC_TRY(get_act(c, tag + ".res_b", B, h, w, 256, 1, &xb, s, sp_res));
-  DVC_TRY(get_act(c, tag + ".res_raw", B, h, w, 256, 0, &raw, s));
-  DVC_TRY(get_act(c, tag + ".res_mid", B, h, w, 256, 1, &mid, s, sp));
+  // three residual blocks (NonlocalNet.py:341-352), ping-pong between two padded buffers; keep_stages gives every block
+  // (.res<i>.raw1 / .mid / .raw2 / .out) and the projection (.proj_raw) buffers of their own, so that tests can read
+  // each stage after the call -- same kernels, same arithmetic
+  const bool keep = c->keep_stages != 0;
+  Act xa = cat, xb, raw, mid, raw2;
+  if (!keep) {
+    DVC_TRY(get_act(c, tag + ".res_b", B, h, w, 256, 1, &xb, s, sp_res));
+    DVC_TRY(get_act(c, tag + ".res_raw", B, h, w, 256, 0, &raw, s));
+    DVC_TRY(get_act(c, tag + ".res_mid", B, h, w, 256, 1, &mid, s, sp));
+    raw2 = raw;
+  }
   double chain_bound = cat_bound;
   for (int i = 0; i < 3; ++i) {
+    if (keep) {
+      const std::string r = tag + ".res" + std::to_string(i);
+      DVC_TRY(get_act(c, r + ".raw1", B, h, w, 256, 0, &raw, s));
+      DVC_TRY(get_act(c, r + ".mid", B, h, w, 256, 1, &mid, s, sp));
+      DVC_TRY(get_act(c, r + ".raw2", B, h, w, 256, 0, &raw2, s));
+      DVC_TRY(get_act(c, r + ".out", B, h, w, 256, 1, &xb, s, sp_res));
+    }
     const std::string base = "layer." + std::to_string(i);
     const ConvW *w1, *w2;
     float sl;
@@ -849,13 +864,13 @@ static int warp_side(dvc_ctx* c, const std::string& tag, const Act n[4], const c
     DVC_TRY(run_xform(c, raw, mid, x1, s));
     ConvOpt o2;
     o2.stats = st2;
-    DVC_TRY(run_conv(c, w2, mid, raw, o2, s));
+    DVC_TRY(run_conv(c, w2, mid, raw2, o2, s));
     XfOpt x2;
     x2.pad_mode = PAD_REFLECT, x2.stats = st2, x2.count = (double)h * w, x2.act = 2, x2.slope = sl, x2.res = &xa;
     // out = PReLU(IN(conv2(..)) + x) (NonlocalNet.py:341-352): |out| <= (sqrt(hw) + |x|max) * max(1, |slope|)
     chain_bound = (chain_bound + sqrt((double)h * w)) * fmax(1.0, fabs(sl));
     xb.e16 = e16_for(chain_bound);
-    DVC_TRY(run_xform(c, raw, xb, x2, s));
+    DVC_TRY(run_xform(c, raw2, xb, x2, s));
     std::swap(xa, xb);
   }
 
@@ -866,6 +881,7 @@ static int warp_side(dvc_ctx* c, const std::string& tag, const Act n[4], const c
   DVC_TRY(stats_alloc(c, B, 256, &stp, s));
   ConvOpt op;
   op.stats = stp;
+  if (keep) DVC_TRY(get_act(c, tag + ".proj_raw", B, h, w, 256, 0, &raw, s));
   DVC_TRY(run_conv(c, wp, xa, raw, op, s));
   DVC_TRY(run_pixnorm(c, raw, rows_out, nullptr, 0, PAD_ZERO, stp, (double)h * w, s));
   return DVC_OK;
@@ -1044,7 +1060,16 @@ static int colorvid(dvc_ctx* c, const std::string& tag, const Act& in0, float* o
 // ------------------------------------------------------------------------------------------------
 // C ABI
 // ------------------------------------------------------------------------------------------------
-static bool legal_shape(int H, int W) { return H >= 16 && W >= 16 && H % 8 == 0 && W % 16 == 0; }
+// Frame shapes the reference runs: the VGG trunk pools four times before r52, which must be at least 2x2 for the fifth
+// max-pool (NonlocalNet.py:255) and for the r5 head's ReflectionPad2d(1); the heads' outputs are concatenated, which
+// needs H % 8 == 0 and W % 16 == 0 (NonlocalNet.py:464).  Checked before anything is launched.
+static int check_frame_shape(dvc_ctx* c, const char* what, int H, int W) {
+  if (H < 32 || W < 32)
+    return fail(c, DVC_ERR_SHAPE, std::string(what) + ": H and W must be >= 32 (the r52 feature map must be at least 2x2)");
+  if (H % 8 || W % 16)
+    return fail(c, DVC_ERR_SHAPE, std::string(what) + ": H must be a multiple of 8 and W a multiple of 16 (the reference fails at NonlocalNet.py:464 otherwise)");
+  return DVC_OK;
+}
 
 extern "C" const char* dvc_version(void) { return "libdvc 0.1 (sm_90a)"; }
 
@@ -1150,6 +1175,7 @@ extern "C" int dvc_debug_set_flag(dvc_ctx* c, const char* name, int value) {
   if (!strcmp(name, "clip_astreams")) { c->clip_astreams = value == 2 ? 2 : 1; return DVC_OK; }
   if (!strcmp(name, "tc_tail")) { c->tc_tail = value < 0 ? 0 : value; return DVC_OK; }  // > 1: pretend pair-slot count (tests)
   if (!strcmp(name, "tc_f16")) { c->tc_f16 = value != 0; return DVC_OK; }
+  if (!strcmp(name, "keep_stages")) { c->keep_stages = value != 0; return DVC_OK; }
   if (!strcmp(name, "tc_splits")) { c->tc_splits = value < 0 ? 0 : (value > 8 ? 8 : value); return DVC_OK; }
   if (!strcmp(name, "tc_kbytes")) { c->tc_kbytes = value == 64 ? 64 : 128; return DVC_OK; }
   if (!strcmp(name, "tc_cluster")) { c->tc_cluster = value == 2 ? 2 : 1; return DVC_OK; }
@@ -1240,7 +1266,8 @@ extern "C" double dvc_corr_mean_ms(dvc_ctx* c, int reset) {
 extern "C" int dvc_vgg19_forward(dvc_ctx* c, const float* x, int B, int H, int W, int preprocess, const char* const* keys,
                                  float* const* outs, int n_keys, void* stream) {
   if (!c || !x || !keys || !outs || B < 1 || n_keys < 1) return c ? fail(c, DVC_ERR_ARG, "vgg19_forward: bad argument") : DVC_ERR_ARG;
-  if (H < 16 || W < 16) return fail(c, DVC_ERR_SHAPE, "vgg19_forward: H, W must be >= 16");
+  // the reference evaluates all five pools; its fifth raises on a 1-pixel input (H or W < 32)
+  if (H < 32 || W < 32) return fail(c, DVC_ERR_SHAPE, "vgg19_forward: H and W must be >= 32 (the fifth max-pool needs a 2x2 input)");
   cudaStream_t s = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->device));
   // deepest requested map decides where the trunk stops (the reference evaluates all 21 stages
@@ -1294,7 +1321,8 @@ static int features_from_nchw(dvc_ctx* c, const std::string& tag, const float* c
   const int hs[4] = {H / 2, H / 4, H / 8, H / 16}, ws[4] = {W / 2, W / 4, W / 8, W / 16}, cs[4] = {128, 256, 512, 512};
   for (int k = 0; k < 4; ++k) {
     DVC_TRY(get_act(c, tag + ".n" + std::to_string(k), B, hs[k], ws[k], cs[k], 1, &n[k], s, tc_mode(c)));
-    launch_nchw_to_act(f[k], cs[k], n[k].d, n[k].lo, B, hs[k], ws[k], cs[k], 1, PAD_REFLECT, 0, s);
+    if (!launch_nchw_to_act(f[k], cs[k], n[k].d, n[k].lo, B, hs[k], ws[k], cs[k], 1, PAD_REFLECT, 0, s))
+      return fail(c, DVC_ERR_SHAPE, "nchw_to_act: reflect pad too wide");
     DVC_TRY(check_launch(c, "nchw_to_act"));
   }
   return DVC_OK;
@@ -1306,7 +1334,7 @@ extern "C" int dvc_warpnet_forward(dvc_ctx* c, const float* B_lab_map, const flo
   if (!c || !B_lab_map || !A || !Bf || !y || !sim || B < 1) return c ? fail(c, DVC_ERR_ARG, "warpnet_forward: bad argument") : DVC_ERR_ARG;
   if (wta != 1.0f) return fail(c, DVC_ERR_ARG, "warpnet_forward: WTA_scale_weight != 1 is not supported (training-only path, NonlocalNet.py:486)");
   if (!(temperature > 0.f)) return fail(c, DVC_ERR_ARG, "warpnet_forward: temperature must be > 0");
-  if (!legal_shape(H, W)) return fail(c, DVC_ERR_SHAPE, "warpnet_forward: H must be a multiple of 8 and W a multiple of 16 (the reference fails at NonlocalNet.py:464 otherwise)");
+  DVC_TRY(check_frame_shape(c, "warpnet_forward", H, W));
   cudaStream_t s = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->device));
   DVC_TRY(stats_begin(c, s));
@@ -1556,7 +1584,7 @@ static int normalised_features(dvc_ctx* c, const std::string& tag, VggMaps& maps
 
 extern "C" int dvc_set_exemplar(dvc_ctx* c, const float* IB_lab, int H, int W, void* stream) {
   if (!c || !IB_lab) return c ? fail(c, DVC_ERR_ARG, "set_exemplar: bad argument") : DVC_ERR_ARG;
-  if (!legal_shape(H, W)) return fail(c, DVC_ERR_SHAPE, "set_exemplar: H must be a multiple of 8 and W a multiple of 16");
+  DVC_TRY(check_frame_shape(c, "set_exemplar", H, W));
   cudaStream_t s = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->device));
   DVC_TRY(stats_begin(c, s));
@@ -1949,7 +1977,7 @@ extern "C" int dvc_exemplar_export(dvc_ctx* c, float* buf, int64_t n, void* stre
 
 extern "C" int dvc_exemplar_import(dvc_ctx* c, const float* buf, int64_t n, int H, int W, void* stream) {
   if (!c || !buf) return c ? fail(c, DVC_ERR_ARG, "exemplar_import: bad argument") : DVC_ERR_ARG;
-  if (!legal_shape(H, W)) return fail(c, DVC_ERR_SHAPE, "exemplar_import: illegal frame shape");
+  DVC_TRY(check_frame_shape(c, "exemplar_import", H, W));
   const int64_t N = (int64_t)(H / 4) * (W / 4);
   if (n != N * 260) return fail(c, DVC_ERR_SHAPE, "exemplar_import: buffer size mismatch");
   cudaStream_t s = (cudaStream_t)stream;

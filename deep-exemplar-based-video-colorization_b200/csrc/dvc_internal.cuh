@@ -162,8 +162,9 @@ void launch_pixnorm(const PixNormParams& p, int B, cudaStream_t s);
 // ---- small layout / helper kernels -------------------------------------------------------------
 // NCHW [B][Cs][H][W] -> padded NHWC with C channels (extra channels zero); mode: 0 copy,
 // 1 rgb -> vgg_preprocess (util.py:347-352), 2 centred L -> gray -> vgg_preprocess (util.py:97-101),
-// 3 centred Lab -> sRGB (util.py:379-414) -> vgg_preprocess
-void launch_nchw_to_act(const float* src, int Cs, float* dst, float* dst_lo, int B, int H, int W, int C, int P,
+// 3 centred Lab -> sRGB (util.py:379-414) -> vgg_preprocess.  Returns false (nothing launched) for a reflect border as
+// wide as the map (P >= H or P >= W).
+bool launch_nchw_to_act(const float* src, int Cs, float* dst, float* dst_lo, int B, int H, int W, int C, int P,
                         int pad_mode, int mode, cudaStream_t s);
 void launch_act_to_nchw(const float* src, const float* src_lo, int H, int W, int P, int sC, int sCoff, int C, float* dst,
                         int B, cudaStream_t s);

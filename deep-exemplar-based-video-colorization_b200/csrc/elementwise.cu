@@ -630,11 +630,13 @@ void launch_pixnorm(const PixNormParams& p, int B, cudaStream_t s) {
   launch_counter_add(1);
 }
 
-void launch_nchw_to_act(const float* src, int Cs, float* dst, float* dst_lo, int B, int H, int W, int C, int P,
+bool launch_nchw_to_act(const float* src, int Cs, float* dst, float* dst_lo, int B, int H, int W, int C, int P,
                         int pad_mode, int mode, cudaStream_t s) {
+  if (pad_mode == PAD_REFLECT && (P >= H || P >= W)) return false;  // reflect_idx would leave the source
   dim3 grid(grid_for((long)(H + 2 * P) * (W + 2 * P), 256), B);
   nchw_to_act_kernel<<<grid, 256, 0, s>>>(src, Cs, dst, dst_lo, H, W, C, P, pad_mode, mode);
   launch_counter_add(1);
+  return true;
 }
 
 void launch_act_to_nchw(const float* src, const float* src_lo, int H, int W, int P, int sC, int sCoff, int C, float* dst,

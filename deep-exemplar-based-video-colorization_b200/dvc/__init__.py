@@ -435,8 +435,12 @@ class Context:
         self._check(rc, "dvc_debug_conv2d")
         return (y, st) if want_stats else y
 
-    def debug_buffer(self, name, act=True):
-        """Copy of an internal workspace.  act=True: padded NHWC activation -> interior as NCHW [B,C,H,W]."""
+    def debug_buffer(self, name, act=True, keep_border=False, fp16=False):
+        """Copy of an internal workspace.  act=True: padded NHWC activation -> interior as NCHW [B,C,H,W].
+
+        keep_border=True returns the padded tensor [B,C,H+2P,W+2P].  An activation stored as fp16 hi/lo planes of
+        value * 2^e comes back as hi + lo in those scaled units (the exponent lives in the layer program); fp16=True
+        asks for those planes also when the buffer keeps an fp32 plane beside them."""
         ptr, nbytes, sig = ctypes.c_void_p(0), ctypes.c_int64(0), (ctypes.c_int * 5)()
         self._check(self.lib.dvc_debug_get_buffer(self.h, name.encode(), ctypes.byref(ptr), ctypes.byref(nbytes), sig),
                     "dvc_debug_get_buffer")
@@ -450,14 +454,17 @@ class Context:
             P = -1 - P
         mode16, P = divmod(P, 1000)  # 2: fp16 hi/lo planes of value * 2^e only; 3: an fp32 plane followed by them
         n = B * (H + 2 * P) * (W + 2 * P) * C
-        if mode16 == 2:
-            # the static exponent lives in the layer program; return hi + lo in scaled units
-            halves = flat.view(torch.float16)
+        if fp16 and mode16 not in (2, 3):
+            raise DvcError(f"debug_buffer({name}): no fp16 planes in this buffer")
+        if mode16 == 2 or (mode16 == 3 and fp16):
+            halves = flat.view(torch.float16)[(2 * n if mode16 == 3 else 0):]
             t = halves[:n].float() + halves[n:2 * n].float()
         else:
             t = flat[:n] + flat[n:2 * n] if split else flat[:n]
         t = t.view(B, H + 2 * P, W + 2 * P, C)
-        return t[:, P:P + H, P:P + W, :].permute(0, 3, 1, 2).contiguous()
+        if not keep_border:
+            t = t[:, P:P + H, P:P + W, :]
+        return t.permute(0, 3, 1, 2).contiguous()
 
     # ---- introspection ---------------------------------------------------------------------------
     def launch_count(self, reset=False):

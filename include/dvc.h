@@ -16,8 +16,9 @@
  *     entry point synchronises the device unless stated.
  *   - there is NO CPU fallback: without a CUDA device every compute entry point fails with
  *     DVC_ERR_CUDA.
- *   - legal frame shapes are the reference's (SURVEY.md fact 2): H % 8 == 0, W % 16 == 0, H,W >= 16;
- *     anything else returns DVC_ERR_SHAPE (the reference raises RuntimeError at NonlocalNet.py:464).
+ *   - legal frame shapes are the reference's (SURVEY.md fact 2): H % 8 == 0, W % 16 == 0, H,W >= 32;
+ *     anything else returns DVC_ERR_SHAPE before any launch (the reference raises RuntimeError at
+ *     NonlocalNet.py:464, or at VGG19's fifth max-pool when the r52 map is narrower than 2x2).
  */
 #ifndef DVC_H_
 #define DVC_H_
@@ -213,7 +214,9 @@ int dvc_conv_profile(dvc_ctx* ctx, int variant, int reset, double* total_ms, dou
 
 /* Debug / test hooks (not part of the drop-in surface).
  *   dvc_debug_set_flag: "two_level" (default 1) selects per-tap two-level fp32 accumulation in the
- *   CUDA-core convolution (shorter rounding chain; 0 = plain sequential accumulation, faster).
+ *   CUDA-core convolution (shorter rounding chain; 0 = plain sequential accumulation, faster).  "keep_stages" (default 0)
+ *   gives WarpNet's residual blocks and projection buffers of their own (<tag>.res<i>.raw1 / .mid / .raw2 / .out,
+ *   <tag>.proj_raw) instead of reusing two, so every stage can be read after the call; results are bit-identical.
  *   dvc_debug_get_buffer: device pointer / size of a named internal workspace (padded NHWC activations
  *   carry their [B,H,W,C,P] signature in sig5) so tests can check intermediate stages.  "corr.screen_cells" is the
  *   screened T -> 0 correlation's 4 maxima (float bits): query-side ||dropped||, ||hi||, then reference-side. */

@@ -373,8 +373,9 @@ def rgb8_to_lab(rgb):
 
 
 def legal_shape(H, W):
-    """Shapes the reference's full path accepts (SURVEY.md fact 2): H % 8 == 0 and W % 16 == 0."""
-    return H % 8 == 0 and W % 16 == 0 and H >= 16 and W >= 16
+    """Shapes the reference's full path accepts (SURVEY.md fact 2): H % 8 == 0 and W % 16 == 0 (NonlocalNet.py:464), and
+    H, W >= 32: below that VGG19's fifth max-pool (NonlocalNet.py:255) gets a 1-pixel input and raises."""
+    return H % 8 == 0 and W % 16 == 0 and H >= 32 and W >= 32
 
 
 def corr_flops(NA, NB, C=256, ch=3):

@@ -86,6 +86,42 @@ def test_legal_shapes():
     assert not legal_shape(480, 854) and not legal_shape(36, 64)
 
 
+def _oracle_frame(sds, H, W):
+    """One fp32 oracle frame (exemplar features included) at H x W."""
+    from oracle import dvc_oracle as O
+    from oracle.weights import make_lab
+
+    IA, IB, last = make_lab(80, 1, H, W), make_lab(81, 1, H, W), make_lab(82, 1, H, W)
+    with torch.no_grad():
+        fB = O.exemplar_features(sds["vgg"], IB)
+        return O.frame_colorization(sds, IA, IB, last, fB)[0]
+
+
+@pytest.mark.parametrize("H,W", [(16, 64), (24, 64), (32, 16)])
+def test_oracle_rejects_frames_below_32(sds, H, W):
+    """The reference cannot run frames whose r52 map is narrower than 2x2: VGG19's fifth max-pool raises."""
+    with pytest.raises(RuntimeError, match="too small"):
+        _oracle_frame(sds, H, W)
+
+
+def test_oracle_runs_smallest_legal_frame(sds):
+    ab = _oracle_frame(sds, 32, 32)
+    assert ab.shape == (1, 2, 32, 32) and torch.isfinite(ab).all()
+
+
+def test_legal_shape_agrees_with_the_oracle(sds):
+    from oracle.dvc_oracle import legal_shape
+
+    for H in (16, 24, 32, 40):
+        for W in (16, 32, 48):
+            try:
+                _oracle_frame(sds, H, W)
+                runs = True
+            except RuntimeError:
+                runs = False
+            assert legal_shape(H, W) == runs, (H, W, runs)
+
+
 _WORKER = r"""
 import os, sys, torch, torch.distributed as dist
 sys.path.insert(0, sys.argv[1]); sys.path.insert(0, sys.argv[2])
