@@ -97,6 +97,7 @@ struct SplitOut {
 
 struct TcParams {
   int NA, NB, B, Bphi, C;
+  int a_bstride;  // query rows between batches in the A planes: NA, or 0 when every batch shares one query set
   int tiles_per_split;
   float sc;  // log2(e) / T
   const float* row_sc;  // optional per-query-row log2(e) / T_i (overrides sc): the contextual loss normalises every row by its own minimum distance
@@ -247,8 +248,8 @@ __global__ void __launch_bounds__(NTHREADS, 1)
           if (tc::elect_one()) {
             uint8_t* st = smem + stage * STAGE_BYTES;
             tc::mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
-            tc::tma_load_2d(st, &tmAh, &full[stage], kb * KB, b * p.NA + m0);
-            tc::tma_load_2d(st + A_BYTES, &tmAl, &full[stage], kb * KB, b * p.NA + m0);
+            tc::tma_load_2d(st, &tmAh, &full[stage], kb * KB, b * p.a_bstride + m0);
+            tc::tma_load_2d(st + A_BYTES, &tmAl, &full[stage], kb * KB, b * p.a_bstride + m0);
             if (CL == 1) {
               tc::tma_load_2d(st + 2 * A_BYTES, &tmBh, &full[stage], kb * KB, col0);
               tc::tma_load_2d(st + 2 * A_BYTES + B_BYTES, &tmBl, &full[stage], kb * KB, col0);
@@ -420,9 +421,10 @@ struct ScreenCfg {
 
 struct ScreenParams {
   int NA, NB, B, Bphi, C;
+  int a_bstride;  // query rows between batches in the A plane and the query norms: NA, or 0 for one shared query set
   int tiles_per_split;
-  const float* nd_a;   // [B*NA]   ||dropped part|| of every query row
-  const float* nh_a;   // [B*NA]   ||hi part||
+  const float* nd_a;   // [B*NA] (one shared query set: [NA])   ||dropped part|| of every query row
+  const float* nh_a;   //                                       ||hi part||
   const unsigned int* nd_b_max;  // float bits: max over reference rows of ||dropped part||
   const unsigned int* nh_b_max;  //             max over reference rows of ||hi part||
   float* pm;     // [parts][B*NA]            screening maximum of the part (true-score units)
@@ -478,7 +480,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
       uint32_t phase = 0;
       if (ntiles > 0 && tc::elect_one()) {  // the query tile: loaded once, resident for the whole sweep
         tc::mbar_arrive_expect_tx(afull, A_RES);
-        for (int kb = 0; kb < nkb; ++kb) tc::tma_load_2d(smem + kb * A_BYTES, &tmAh, afull, kb * KB, b * p.NA + m0);
+        for (int kb = 0; kb < nkb; ++kb) tc::tma_load_2d(smem + kb * A_BYTES, &tmAh, afull, kb * KB, b * p.a_bstride + m0);
       }
       __syncwarp();
       for (int t = 0; t < ntiles; ++t) {
@@ -516,7 +518,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
     int cnt[2] = {0, 0};  // entries appended (only the first SCREEN_K are stored: cnt > SCREEN_K = overflow)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {  // candidate threshold in accumulator units (scores there are true scores * 2^28)
-      const size_t grow = (size_t)b * p.NA + min(m0 + rl + 8 * h, p.NA - 1);
+      const size_t grow = (size_t)b * p.a_bstride + min(m0 + rl + 8 * h, p.NA - 1);
       thr[h] = screen_threshold(__ldg(p.nd_a + grow), __ldg(p.nh_a + grow), __uint_as_float(__ldg(p.nd_b_max)),
                                 __uint_as_float(__ldg(p.nh_b_max))) * 268435456.0f;
     }
@@ -612,8 +614,9 @@ __global__ void __launch_bounds__(256) corr_rescore_kernel(const float* __restri
   const int bphi = (p.Bphi == 1) ? 0 : b;
   const float* ph = phi + (size_t)bphi * p.NB * 256;
   const float4* Vg = V + (size_t)bphi * p.NB;
-  const float4 a0 = __ldg(reinterpret_cast<const float4*>(theta + (size_t)r * 256) + lane);
-  const float4 a1 = __ldg(reinterpret_cast<const float4*>(theta + (size_t)r * 256) + 32 + lane);
+  const int ra = b * p.a_bstride + (r - b * p.NA);  // query row in theta and in the query norms
+  const float4 a0 = __ldg(reinterpret_cast<const float4*>(theta + (size_t)ra * 256) + lane);
+  const float4 a1 = __ldg(reinterpret_cast<const float4*>(theta + (size_t)ra * 256) + 32 + lane);
   auto score = [&](int col) {
     const float4 b0 = __ldg(reinterpret_cast<const float4*>(ph + (size_t)col * 256) + lane);
     const float4 b1 = __ldg(reinterpret_cast<const float4*>(ph + (size_t)col * 256) + 32 + lane);
@@ -628,7 +631,7 @@ __global__ void __launch_bounds__(256) corr_rescore_kernel(const float* __restri
   };
   float pmax = -INFINITY;
   for (int s = 0; s < nparts; ++s) pmax = fmaxf(pmax, __ldg(p.pm + (size_t)s * rows + r));
-  const float thr = screen_threshold(__ldg(p.nd_a + r), __ldg(p.nh_a + r), __uint_as_float(__ldg(p.nd_b_max)), __uint_as_float(__ldg(p.nh_b_max)));
+  const float thr = screen_threshold(__ldg(p.nd_a + ra), __ldg(p.nh_a + ra), __uint_as_float(__ldg(p.nd_b_max)), __uint_as_float(__ldg(p.nh_b_max)));
   float m = -INFINITY, cnt = 0.f, t0 = 0.f, t1 = 0.f, t2 = 0.f;
   int idx = 0x7fffffff;
   auto visit = [&](int col) {
@@ -827,7 +830,10 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
   const int fmt = math == 1 ? 0 : (math == 2 ? 1 : 2);  // DVC_MATH_TF32X3 / BF16X3 / FP16X3
   if (p.C < 64 || p.C % 64 || p.C > 4096) return fail("C must be a multiple of 64 (<= 4096)");
   const int eb = tf32 ? 4 : 2;
-  const size_t ea = (size_t)p.B * p.NA * p.C, ephi = (size_t)p.Bphi * p.NB * p.C;
+  if (p.theta_shared && p.Bphi != p.B) return fail("a shared query set needs Bphi == B");
+  // query rows in theta / the A planes: one set for all batches when it is shared (prepared once, not B times)
+  const int qrows = (p.theta_shared ? 1 : p.B) * p.NA, a_bstride = p.theta_shared ? 0 : p.NA;
+  const size_t ea = (size_t)qrows * p.C, ephi = (size_t)p.Bphi * p.NB * p.C;
   void *Ah, *Al, *Bh, *Bl, *part;
   if (ws_get(ws, 0, ea * eb, &Ah) || ws_get(ws, 1, ea * eb, &Al) || ws_get(ws, 2, ephi * eb, &Bh) || ws_get(ws, 3, ephi * eb, &Bl))
     return fail("workspace allocation failed");
@@ -873,15 +879,15 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
     const bool phi_cached = phi_version >= 0 && ws->phi_src == p.phi && ws->phi_version == phi_version && ws->phi_fmt == 3 &&
                             ws->phi_elems == ephi;
     if (cudaMemsetAsync(cells, 0, (phi_cached ? 2 : 4) * sizeof(unsigned int), s) != cudaSuccess) return fail("cudaMemsetAsync failed");
-    screen_planes_kernel<<<(rows * 32 + 255) / 256, 256, 0, s>>>(p.theta, (__half*)Ah, nd_a, nh_a, cells + 0, cells + 1, rows);
+    screen_planes_kernel<<<(qrows * 32 + 255) / 256, 256, 0, s>>>(p.theta, (__half*)Ah, nd_a, nh_a, cells + 0, cells + 1, qrows);
     if (!phi_cached) screen_planes_kernel<<<(rphi * 32 + 255) / 256, 256, 0, s>>>(p.phi, (__half*)Bh, nd_b, nh_b, cells + 2, cells + 3, rphi);
     launch_counter_add(phi_cached ? 1 : 2);
     ws->phi_src = phi_version >= 0 ? p.phi : nullptr, ws->phi_version = phi_version, ws->phi_fmt = 3, ws->phi_elems = ephi;
     CUtensorMap mA, mB;
-    if (encode_tmap_2d(&mA, Ah, (uint64_t)rows, p.C, BM, 64, 2) || encode_tmap_2d(&mB, Bh, (uint64_t)rphi, p.C, BN / cl, 64, 2))
+    if (encode_tmap_2d(&mA, Ah, (uint64_t)qrows, p.C, BM, 64, 2) || encode_tmap_2d(&mB, Bh, (uint64_t)rphi, p.C, BN / cl, 64, 2))
       return fail("cuTensorMapEncodeTiled failed");
     ScreenParams sp;
-    sp.NA = p.NA, sp.NB = p.NB, sp.B = p.B, sp.Bphi = p.Bphi, sp.C = p.C, sp.tiles_per_split = tps;
+    sp.NA = p.NA, sp.NB = p.NB, sp.B = p.B, sp.Bphi = p.Bphi, sp.C = p.C, sp.a_bstride = a_bstride, sp.tiles_per_split = tps;
     sp.nd_a = nd_a, sp.nh_a = nh_a, sp.nd_b_max = cells + 2, sp.nh_b_max = cells + 3;
     sp.pm = (float*)cand;
     sp.pcnt = (int*)(sp.pm + (size_t)sparts * rows);
@@ -916,13 +922,13 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
 
   CUtensorMap mAh, mAl, mBh, mBl;
   const uint32_t boxk = tf32 ? 32 : 64;
-  if (encode_tmap_2d(&mAh, Ah, (uint64_t)p.B * p.NA, p.C, BM, boxk, eb) || encode_tmap_2d(&mAl, Al, (uint64_t)p.B * p.NA, p.C, BM, boxk, eb) ||
+  if (encode_tmap_2d(&mAh, Ah, (uint64_t)qrows, p.C, BM, boxk, eb) || encode_tmap_2d(&mAl, Al, (uint64_t)qrows, p.C, BM, boxk, eb) ||
       encode_tmap_2d(&mBh, Bh, (uint64_t)p.Bphi * p.NB, p.C, BN / cl, boxk, eb) ||
       encode_tmap_2d(&mBl, Bl, (uint64_t)p.Bphi * p.NB, p.C, BN / cl, boxk, eb))
     return fail("cuTensorMapEncodeTiled failed");
 
   TcParams tp;
-  tp.NA = p.NA, tp.NB = p.NB, tp.B = p.B, tp.Bphi = p.Bphi, tp.C = p.C, tp.tiles_per_split = tps;
+  tp.NA = p.NA, tp.NB = p.NB, tp.B = p.B, tp.Bphi = p.Bphi, tp.C = p.C, tp.a_bstride = a_bstride, tp.tiles_per_split = tps;
   tp.sc = 1.4426950408889634f / p.temperature;
   tp.row_sc = p.row_scale;
   tp.out_scale = fmt == 2 ? 3.725290298461914e-09f /* 2^-28 */ : 1.0f;

@@ -164,10 +164,10 @@ struct dvc_ctx {
   cudaEvent_t evA[4] = {nullptr, nullptr, nullptr, nullptr}, evC[4] = {nullptr, nullptr, nullptr, nullptr}, evFork = nullptr,
               evJoinA = nullptr, evJoinC = nullptr, evJoinD = nullptr;
   cudaEvent_t evU[4] = {nullptr, nullptr, nullptr, nullptr}, evD[4] = {nullptr, nullptr, nullptr, nullptr};
-  // exemplar cache
-  float* ex_phi = nullptr;  // [N][256]
-  float* ex_V = nullptr;    // [N][4]
-  int ex_H = 0, ex_W = 0, ex_N = 0;
+  // exemplar cache: ex_K slots (dvc_set_exemplars; 1 after dvc_set_exemplar / dvc_exemplar_import), room for ex_slots
+  float* ex_phi = nullptr;  // [K][N][256]
+  float* ex_V = nullptr;    // [K][N][4]
+  int ex_H = 0, ex_W = 0, ex_N = 0, ex_K = 1, ex_slots = 0;
   bool ex_valid = false;
   // module-level WarpNet B-side cache
   bool warp_cache_valid = false;
@@ -1474,23 +1474,26 @@ extern "C" int dvc_debug_conv2d(dvc_ctx* c, int net, const char* name, const flo
 }
 
 // ---- stand-alone correlation ---------------------------------------------------------------------
-extern "C" int dvc_corr_softmax_warp(dvc_ctx* c, const float* theta_hat, const float* phi_hat, const float* V, int B,
-                                     int Bphi, int NA, int NB, int C, float temperature, float* y, float* sim,
-                                     int32_t* argmax, void* stream) {
+// theta_shared: one query set [1][C][NA] against B = Bphi reference sets (dvc_corr_softmax_warp_exemplars)
+static int corr_standalone(dvc_ctx* c, const float* theta_hat, const float* phi_hat, const float* V, int B, int Bphi,
+                           bool theta_shared, int NA, int NB, int C, float temperature, float* y, float* sim, int32_t* argmax,
+                           void* stream) {
   if (!c || !theta_hat || !phi_hat || !V || !y || !sim) return c ? fail(c, DVC_ERR_ARG, "corr: bad argument") : DVC_ERR_ARG;
   if (C < 64 || C % 64 || C > 4096) return fail(c, DVC_ERR_SHAPE, "corr: C must be a multiple of 64 (WarpNet.inter_channels is 256)");
   if (C != 256 && c->corr_math == DVC_MATH_FP32) return fail(c, DVC_ERR_SHAPE, "corr: the CUDA-core twin is built for C = 256");
   if (B < 1 || NA < 1 || NB < 1 || (Bphi != B && Bphi != 1)) return fail(c, DVC_ERR_SHAPE, "corr: bad sizes");
   if (!(temperature > 0.f)) return fail(c, DVC_ERR_ARG, "corr: temperature must be > 0");
+  if (theta_shared && c->corr_peers.n > 0) return fail(c, DVC_ERR_STATE, "corr: peer outputs are not supported with several exemplars");
   cudaStream_t s = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->device));
+  const int Bq = theta_shared ? 1 : B;  // query sets
   void *th, *ph, *V4, *y4;
-  DVC_TRY(get_raw(c, "corr.theta", (size_t)B * NA * C * 4, &th, s));
+  DVC_TRY(get_raw(c, "corr.theta", (size_t)Bq * NA * C * 4, &th, s));
   DVC_TRY(get_raw(c, "corr.phi", (size_t)Bphi * NB * C * 4, &ph, s));
   DVC_TRY(get_raw(c, "corr.V4", (size_t)Bphi * NB * 16, &V4, s));
   DVC_TRY(get_raw(c, "corr.y4", (size_t)B * NA * 16, &y4, s));
   // channel-major [b][C][N] (the reference's view, NonlocalNet.py:468,473) -> position-major rows
-  launch_transpose_cn(theta_hat, (float*)th, B, C, NA, s);
+  launch_transpose_cn(theta_hat, (float*)th, Bq, C, NA, s);
   const long long dims = ((long long)Bphi << 40) ^ ((long long)NB << 8) ^ C;
   const bool phi_ready = c->corr_phi_static && c->corr_phi_key == phi_hat && c->corr_V_key == V && c->corr_phi_dims == dims;
   if (!phi_ready) {
@@ -1502,6 +1505,7 @@ extern "C" int dvc_corr_softmax_warp(dvc_ctx* c, const float* theta_hat, const f
   }
   CorrParams p{};
   p.theta = (float*)th, p.phi = (float*)ph, p.V = (float*)V4, p.B = B, p.Bphi = Bphi, p.NA = NA, p.NB = NB, p.C = C;
+  p.theta_shared = theta_shared;
   p.temperature = temperature, p.y = (float*)y4, p.sim = sim, p.argmax = argmax;
   if (c->corr_peers.n > 0) {
     if (B != 1) return fail(c, DVC_ERR_SHAPE, "corr: peer outputs need B = 1");
@@ -1512,6 +1516,19 @@ extern "C" int dvc_corr_softmax_warp(dvc_ctx* c, const float* theta_hat, const f
   DVC_TRY(run_corr(c, p, s, c->corr_phi_static ? (1ll << 40) + c->corr_phi_version : -1));
   CUDA_TRY(c, cudaMemcpy2DAsync(y, 12, y4, 16, 12, (size_t)B * NA, cudaMemcpyDeviceToDevice, s));
   return DVC_OK;
+}
+
+extern "C" int dvc_corr_softmax_warp(dvc_ctx* c, const float* theta_hat, const float* phi_hat, const float* V, int B,
+                                     int Bphi, int NA, int NB, int C, float temperature, float* y, float* sim,
+                                     int32_t* argmax, void* stream) {
+  return corr_standalone(c, theta_hat, phi_hat, V, B, Bphi, false, NA, NB, C, temperature, y, sim, argmax, stream);
+}
+
+extern "C" int dvc_corr_softmax_warp_exemplars(dvc_ctx* c, const float* theta_hat, const float* phi_hat, const float* V, int K,
+                                               int NA, int NB, int C, float temperature, float* y, float* sim, int32_t* argmax,
+                                               void* stream) {
+  if (c && (K < 1 || K > 8)) return fail(c, DVC_ERR_ARG, "corr_exemplars: K must be in [1, 8]");
+  return corr_standalone(c, theta_hat, phi_hat, V, K, K, true, NA, NB, C, temperature, y, sim, argmax, stream);
 }
 
 // ---- query-row-sharded correlation: peer-mapped result buffers (CUDA IPC between the per-GPU processes) -----------
@@ -1582,11 +1599,22 @@ static int normalised_features(dvc_ctx* c, const std::string& tag, VggMaps& maps
   return DVC_OK;
 }
 
-extern "C" int dvc_set_exemplar(dvc_ctx* c, const float* IB_lab, int H, int W, void* stream) {
-  if (!c || !IB_lab) return c ? fail(c, DVC_ERR_ARG, "set_exemplar: bad argument") : DVC_ERR_ARG;
-  DVC_TRY(check_frame_shape(c, "set_exemplar", H, W));
-  cudaStream_t s = (cudaStream_t)stream;
-  CUDA_TRY(c, cudaSetDevice(c->device));
+// room for K exemplar slots of N positions each (the buffers only grow in slots; a new N reallocates)
+static int ex_alloc(dvc_ctx* c, int K, int N) {
+  if (c->ex_N != N || c->ex_slots < K) {
+    if (c->ex_phi) cudaFree(c->ex_phi);
+    if (c->ex_V) cudaFree(c->ex_V);
+    c->ex_phi = c->ex_V = nullptr;
+    c->ex_N = 0, c->ex_slots = 0;
+    CUDA_TRY(c, cudaMalloc((void**)&c->ex_phi, (size_t)K * N * 256 * 4));
+    CUDA_TRY(c, cudaMalloc((void**)&c->ex_V, (size_t)K * N * 16));
+    c->ex_N = N, c->ex_slots = K;
+  }
+  return DVC_OK;
+}
+
+// Exemplar prologue (test.py:57-66) of one exemplar IB_lab [1,3,H,W] into phi [N][256] / V [N][4]
+static int exemplar_prologue(dvc_ctx* c, const float* IB_lab, int H, int W, float* phi, float* V, cudaStream_t s) {
   DVC_TRY(stats_begin(c, s));
   void* lab;
   DVC_TRY(get_raw(c, "ex.lab", (size_t)3 * H * W * 4, &lab, s));
@@ -1599,27 +1627,49 @@ extern "C" int dvc_set_exemplar(dvc_ctx* c, const float* IB_lab, int H, int W, v
   DVC_TRY(vgg_trunk(c, "ex", x0, "r52", &maps, s));
   Act n[4];
   DVC_TRY(normalised_features(c, "ex", maps, n, s));
-  const int h = H / 4, w = W / 4, N = h * w;
-  if (c->ex_N != N) {
-    if (c->ex_phi) cudaFree(c->ex_phi);
-    if (c->ex_V) cudaFree(c->ex_V);
-    c->ex_phi = c->ex_V = nullptr;
-    CUDA_TRY(c, cudaMalloc((void**)&c->ex_phi, (size_t)N * 256 * 4));
-    CUDA_TRY(c, cudaMalloc((void**)&c->ex_V, (size_t)N * 16));
-    c->ex_N = N;
-  }
-  DVC_TRY(warp_side(c, "ex", n, "phi", c->ex_phi, h, w, s));
-  launch_avgpool4_lab((float*)lab, c->ex_V, 1, H, W, s);
-  DVC_TRY(check_launch(c, "avgpool4"));
-  c->ex_H = H, c->ex_W = W, c->ex_valid = true, c->ex_version++;
+  DVC_TRY(warp_side(c, "ex", n, "phi", phi, H / 4, W / 4, s));
+  launch_avgpool4_lab((float*)lab, V, 1, H, W, s);
+  return check_launch(c, "avgpool4");
+}
+
+extern "C" int dvc_set_exemplar(dvc_ctx* c, const float* IB_lab, int H, int W, void* stream) {
+  if (!c || !IB_lab) return c ? fail(c, DVC_ERR_ARG, "set_exemplar: bad argument") : DVC_ERR_ARG;
+  DVC_TRY(check_frame_shape(c, "set_exemplar", H, W));
+  cudaStream_t s = (cudaStream_t)stream;
+  CUDA_TRY(c, cudaSetDevice(c->device));
+  const int N = (H / 4) * (W / 4);
+  DVC_TRY(ex_alloc(c, 1, N));
+  DVC_TRY(exemplar_prologue(c, IB_lab, H, W, c->ex_phi, c->ex_V, s));
+  c->ex_H = H, c->ex_W = W, c->ex_K = 1, c->ex_valid = true, c->ex_version++;
   // the frame loop must not allocate: size the correlation workspace for one frame against this exemplar now
   if (corr_ws_reserve(&c->corr_ws, 1, 1, N, N) != 0) return fail(c, DVC_ERR_CUDA, "set_exemplar: correlation workspace allocation failed");
   return DVC_OK;
 }
 
+// K exemplars: dvc_set_exemplar's prologue once per exemplar into slot k, so that every slot holds exactly the bits
+// dvc_set_exemplar gives that exemplar (a batched prologue would share the device-derived fp16 scales and the
+// InstanceNorm summation order across exemplars)
+extern "C" int dvc_set_exemplars(dvc_ctx* c, const float* IB_lab, int K, int H, int W, void* stream) {
+  if (!c || !IB_lab) return c ? fail(c, DVC_ERR_ARG, "set_exemplars: bad argument") : DVC_ERR_ARG;
+  if (K < 1 || K > 8) return fail(c, DVC_ERR_ARG, "set_exemplars: K must be in [1, 8]");
+  DVC_TRY(check_frame_shape(c, "set_exemplars", H, W));
+  cudaStream_t s = (cudaStream_t)stream;
+  CUDA_TRY(c, cudaSetDevice(c->device));
+  const int N = (H / 4) * (W / 4);
+  c->ex_valid = false;  // until every slot is written
+  DVC_TRY(ex_alloc(c, K, N));
+  for (int k = 0; k < K; ++k)
+    DVC_TRY(exemplar_prologue(c, IB_lab + (size_t)k * 3 * H * W, H, W, c->ex_phi + (size_t)k * N * 256, c->ex_V + (size_t)k * N * 4, s));
+  c->ex_H = H, c->ex_W = W, c->ex_K = K, c->ex_valid = true, c->ex_version++;
+  // one frame against K exemplars: K output rows per query row
+  if (corr_ws_reserve(&c->corr_ws, K, K, N, N) != 0) return fail(c, DVC_ERR_CUDA, "set_exemplars: correlation workspace allocation failed");
+  return DVC_OK;
+}
+
 // Phase A (independent of the previous frame): VGG19 -> feature_normalize -> WarpNet A side -> correlation.
+// K > 1 (B = 1): the frame's theta against each of the K cached exemplars, into K rows of yrows / simrows.
 static int frames_phaseA(dvc_ctx* c, const std::string& tag, const float* IA_l, int B, int H, int W, float temperature,
-                         float* yrows, float* simrows, cudaStream_t s, int arena = 0, CorrWorkspace* ws = nullptr) {
+                         float* yrows, float* simrows, cudaStream_t s, int arena = 0, CorrWorkspace* ws = nullptr, int K = 1) {
   DVC_TRY(stats_begin(c, s, arena));
   const int h = H / 4, w = W / 4, N = h * w;
   Act x0;
@@ -1634,24 +1684,33 @@ static int frames_phaseA(dvc_ctx* c, const std::string& tag, const float* IA_l, 
   DVC_TRY(get_raw(c, tag + ".theta", (size_t)B * N * 256 * 4, &theta, s));
   DVC_TRY(warp_side(c, tag, n, "theta", (float*)theta, h, w, s));
   CorrParams p{};
-  p.theta = (float*)theta, p.phi = c->ex_phi, p.V = c->ex_V, p.B = B, p.Bphi = 1, p.NA = N, p.NB = N, p.C = 256;
+  p.theta = (float*)theta, p.phi = c->ex_phi, p.V = c->ex_V, p.B = K > 1 ? K : B, p.Bphi = K, p.NA = N, p.NB = N, p.C = 256;
+  p.theta_shared = K > 1;
   p.temperature = temperature, p.y = yrows, p.sim = simrows, p.argmax = nullptr;
   return run_corr(c, p, s, c->ex_version, ws);
 }
 
 // Phase C (the recurrent part): ColorVidNet on [L, warped ab, similarity, previous Lab] (FrameColor.py:63-65).
+// l_bstride: floats between the L planes of consecutive batches (0: one frame's L for all K exemplars' recurrences)
 static int frames_phaseC(dvc_ctx* c, const std::string& tag, const float* IA_l, const float* yrows, const float* simrows,
-                         const float* IA_last_lab, int B, int H, int W, float* out_ab, cudaStream_t s) {
+                         const float* IA_last_lab, int B, int H, int W, float* out_ab, cudaStream_t s, size_t l_bstride) {
   DVC_TRY(stats_begin(c, s, 1));
   Act in0;
   DVC_TRY(get_act(c, tag + ".in0", B, H, W, 8, 1, &in0, s));
-  launch_build_color_input(IA_l, yrows, simrows, IA_last_lab, in0.d, B, H, W, 1, s);
+  launch_build_color_input(IA_l, l_bstride, yrows, simrows, IA_last_lab, in0.d, B, H, W, 1, s);
   DVC_TRY(check_launch(c, "build_color_input"));
   return colorvid(c, tag, in0, out_ab, s);
 }
 
-static int check_frame_args(dvc_ctx* c, int H, int W, float temperature) {
+// K: number of exemplars the call runs against; 0 for the single-exemplar entry points, which refuse a multi-slot cache
+// rather than silently using slot 0
+static int check_frame_args(dvc_ctx* c, int H, int W, float temperature, int K = 0) {
   if (!c->ex_valid) return fail(c, DVC_ERR_STATE, "colorize: call dvc_set_exemplar first");
+  if (K == 0 && c->ex_K != 1)
+    return fail(c, DVC_ERR_STATE, "colorize: " + std::to_string(c->ex_K) + " exemplars are cached: use dvc_colorize_frames_exemplars / "
+                "dvc_colorize_clip_exemplars, or dvc_set_exemplar for a single one");
+  if (K != 0 && K != c->ex_K)
+    return fail(c, DVC_ERR_SHAPE, "colorize_exemplars: K = " + std::to_string(K) + " but " + std::to_string(c->ex_K) + " exemplars are cached");
   if (H != c->ex_H || W != c->ex_W) return fail(c, DVC_ERR_SHAPE, "colorize: frame size differs from the exemplar's");
   if (!(temperature > 0.f)) return fail(c, DVC_ERR_ARG, "colorize: temperature must be > 0");
   return DVC_OK;
@@ -1672,7 +1731,28 @@ extern "C" int dvc_colorize_frames(dvc_ctx* c, const float* IA_l, const float* I
     launch_rows_to_nchw_up4((float*)yrows, (float*)simrows, out_warp_lab, out_sim, B, h, w, s);
     DVC_TRY(check_launch(c, "rows_to_nchw_up4"));
   }
-  return frames_phaseC(c, "fr", IA_l, (float*)yrows, (float*)simrows, IA_last_lab, B, H, W, out_ab, s);
+  return frames_phaseC(c, "fr", IA_l, (float*)yrows, (float*)simrows, IA_last_lab, B, H, W, out_ab, s, (size_t)H * W);
+}
+
+// One frame against the K cached exemplars: phase A once at B = 1, the correlation against the K slots, phase C at
+// B = K with the frame's L shared by the K batches.
+extern "C" int dvc_colorize_frames_exemplars(dvc_ctx* c, const float* IA_l, const float* last_lab, int K, int H, int W,
+                                             float temperature, float* out_ab, float* out_warp_lab, float* out_sim, void* stream) {
+  if (!c || !IA_l || !last_lab || !out_ab) return c ? fail(c, DVC_ERR_ARG, "colorize_frames_exemplars: bad argument") : DVC_ERR_ARG;
+  if (K < 1 || K > 8) return fail(c, DVC_ERR_ARG, "colorize_frames_exemplars: K must be in [1, 8]");
+  DVC_TRY(check_frame_args(c, H, W, temperature, K));
+  cudaStream_t s = (cudaStream_t)stream;
+  CUDA_TRY(c, cudaSetDevice(c->device));
+  const int h = H / 4, w = W / 4, N = h * w;
+  void *yrows, *simrows;
+  DVC_TRY(get_raw(c, "frx.yrows", (size_t)K * N * 16, &yrows, s));
+  DVC_TRY(get_raw(c, "frx.simrows", (size_t)K * N * 4, &simrows, s));
+  DVC_TRY(frames_phaseA(c, "fr", IA_l, 1, H, W, temperature, (float*)yrows, (float*)simrows, s, 0, nullptr, K));
+  if (out_warp_lab || out_sim) {
+    launch_rows_to_nchw_up4((float*)yrows, (float*)simrows, out_warp_lab, out_sim, K, h, w, s);
+    DVC_TRY(check_launch(c, "rows_to_nchw_up4"));
+  }
+  return frames_phaseC(c, "frx", IA_l, (float*)yrows, (float*)simrows, last_lab, K, H, W, out_ab, s, 0);
 }
 
 static int clip_streams(dvc_ctx* c) {
@@ -1701,10 +1781,17 @@ static int clip_streams(dvc_ctx* c) {
 // partial waves of either leave SMs idle that the other fills.  Uploads of L (up to four frames ahead) and downloads
 // of ab run on two copy streams so that neither compute stream ever waits for PCIe.  L / ab may be host (pinned) or
 // device memory.
-extern "C" int dvc_colorize_clip(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature,
-                                 const float* first_last, float* ab_out, void* stream) {
-  if (!c || !L_in || !ab_out || F < 1) return c ? fail(c, DVC_ERR_ARG, "colorize_clip: bad argument") : DVC_ERR_ARG;
-  DVC_TRY(check_frame_args(c, H, W, temperature));
+// K = 0: dvc_colorize_clip (one exemplar); K >= 1: dvc_colorize_clip_exemplars, K recurrences sharing the luminance
+// sequence -- phase A once per frame against the K slots, phase C at batch K, and ab of exemplar k, frame t at
+// ab_out + (k F + t) 2 H W.  The multi-exemplar workspaces have tags of their own, so alternating does not reallocate.
+static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature, const float* first_last,
+                              int K, float* ab_out, void* stream) {
+  const char* what = K ? "colorize_clip_exemplars" : "colorize_clip";
+  if (!c || !L_in || !ab_out || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
+  if (K < 0 || K > 8) return fail(c, DVC_ERR_ARG, std::string(what) + ": K must be in [1, 8]");
+  DVC_TRY(check_frame_args(c, H, W, temperature, K));
+  const int Kb = K ? K : 1;  // batch of phase C
+  const std::string tag = K ? "clipx" : "clip";
   cudaStream_t s = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->device));
   DVC_TRY(clip_streams(c));
@@ -1712,17 +1799,17 @@ extern "C" int dvc_colorize_clip(dvc_ctx* c, const float* L_in, int F, int H, in
   const int N = (H / 4) * (W / 4);
   void *dL, *dlast, *dab, *yrows, *simrows;
   DVC_TRY(get_raw(c, "clip.L", 4 * hw * 4, &dL, s));   // 4 slots
-  DVC_TRY(get_raw(c, "clip.last", 3 * hw * 4, &dlast, s));
-  DVC_TRY(get_raw(c, "clip.ab", 2 * 2 * hw * 4, &dab, s));  // 2 slots
-  DVC_TRY(get_raw(c, "clip.yrows", (size_t)4 * N * 16, &yrows, s));  // 4 slots: phase A may run up to 3 frames ahead
-  DVC_TRY(get_raw(c, "clip.simrows", (size_t)4 * N * 4, &simrows, s));
+  DVC_TRY(get_raw(c, tag + ".last", Kb * 3 * hw * 4, &dlast, s));
+  DVC_TRY(get_raw(c, tag + ".ab", 2 * Kb * 2 * hw * 4, &dab, s));  // 2 slots
+  DVC_TRY(get_raw(c, tag + ".yrows", (size_t)4 * Kb * N * 16, &yrows, s));  // 4 slots: phase A may run up to 3 frames ahead
+  DVC_TRY(get_raw(c, tag + ".simrows", (size_t)4 * Kb * N * 4, &simrows, s));
   const bool two_a = c->clip_astreams == 2;
   // the second phase-A stream has its own correlation workspace (sized like the first at dvc_set_exemplar time)
-  if (two_a && corr_ws_reserve(&c->corr_ws2, 1, 1, N, N) != 0) return fail(c, DVC_ERR_CUDA, "colorize_clip: correlation workspace allocation failed");
+  if (two_a && corr_ws_reserve(&c->corr_ws2, Kb, Kb, N, N) != 0) return fail(c, DVC_ERR_CUDA, std::string(what) + ": correlation workspace allocation failed");
   if (first_last)
-    CUDA_TRY(c, cudaMemcpyAsync(dlast, first_last, 3 * hw * 4, cudaMemcpyDefault, s));
+    CUDA_TRY(c, cudaMemcpyAsync(dlast, first_last, Kb * 3 * hw * 4, cudaMemcpyDefault, s));
   else
-    CUDA_TRY(c, cudaMemsetAsync(dlast, 0, 3 * hw * 4, s));  // test.py:80
+    CUDA_TRY(c, cudaMemsetAsync(dlast, 0, Kb * 3 * hw * 4, s));  // test.py:80
   // Every exit below goes through the join epilogue: an error in the middle of the loop must not return while copies
   // or kernels of earlier frames are still writing into ab_out / the slots (a retry would race with them).
   auto enqueue = [&]() -> int {
@@ -1735,9 +1822,9 @@ extern "C" int dvc_colorize_clip(dvc_ctx* c, const float* L_in, int F, int H, in
     for (int t = 0; t < F; ++t) {
       const int slot = t & 1;
       float* Lt = (float*)dL + (size_t)(t & 3) * hw;
-      float* abt = (float*)dab + (size_t)slot * 2 * hw;
-      float* yr = (float*)yrows + (size_t)(t & 3) * N * 4;
-      float* sr = (float*)simrows + (size_t)(t & 3) * N;
+      float* abt = (float*)dab + (size_t)slot * Kb * 2 * hw;
+      float* yr = (float*)yrows + (size_t)(t & 3) * Kb * N * 4;
+      float* sr = (float*)simrows + (size_t)(t & 3) * Kb * N;
       const bool odd = two_a && (t & 1);
       cudaStream_t sAt = odd ? c->sA2 : c->sA;
       // ---- upload stream: the L slot was last read by frame t-4's ColorVidNet / make_last ----
@@ -1748,18 +1835,20 @@ extern "C" int dvc_colorize_clip(dvc_ctx* c, const float* L_in, int F, int H, in
       // warp-row slot waits for frame t-4's ColorVidNet ----
       CUDA_TRY(c, cudaStreamWaitEvent(sAt, c->evU[t & 3], 0));
       if (t >= 4) CUDA_TRY(c, cudaStreamWaitEvent(sAt, c->evC[(t - 4) & 3], 0));
-      DVC_TRY(frames_phaseA(c, odd ? "clipA2" : "clipA", Lt, 1, H, W, temperature, yr, sr, sAt, odd ? 2 : 0, odd ? &c->corr_ws2 : nullptr));
+      DVC_TRY(frames_phaseA(c, odd ? "clipA2" : "clipA", Lt, 1, H, W, temperature, yr, sr, sAt, odd ? 2 : 0, odd ? &c->corr_ws2 : nullptr,
+                            Kb));
       CUDA_TRY(c, cudaEventRecord(c->evA[t & 3], sAt));
-      // ---- stream C: the recurrent phase ----
+      // ---- stream C: the recurrent phase (the K recurrences read the frame's one L plane) ----
       CUDA_TRY(c, cudaStreamWaitEvent(c->sC, c->evA[t & 3], 0));
       if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sC, c->evD[(t - 2) & 3], 0));  // the ab slot has been downloaded
-      DVC_TRY(frames_phaseC(c, "clipC", Lt, yr, sr, (float*)dlast, 1, H, W, abt, c->sC));
-      launch_make_last(Lt, abt, (float*)dlast, 1, H, W, c->sC);  // test.py:96
+      DVC_TRY(frames_phaseC(c, K ? "clipCx" : "clipC", Lt, yr, sr, (float*)dlast, Kb, H, W, abt, c->sC, 0));
+      launch_make_last(Lt, 0, abt, (float*)dlast, Kb, H, W, c->sC);  // test.py:96
       DVC_TRY(check_launch(c, "make_last"));
       CUDA_TRY(c, cudaEventRecord(c->evC[t & 3], c->sC));
       // ---- download stream ----
       CUDA_TRY(c, cudaStreamWaitEvent(c->sD, c->evC[t & 3], 0));
-      CUDA_TRY(c, cudaMemcpyAsync(ab_out + (size_t)t * 2 * hw, abt, 2 * hw * 4, cudaMemcpyDefault, c->sD));
+      for (int k = 0; k < Kb; ++k)
+        CUDA_TRY(c, cudaMemcpyAsync(ab_out + ((size_t)k * F + t) * 2 * hw, abt + (size_t)k * 2 * hw, 2 * hw * 4, cudaMemcpyDefault, c->sD));
       CUDA_TRY(c, cudaEventRecord(c->evD[t & 3], c->sD));
     }
     return DVC_OK;
@@ -1782,9 +1871,20 @@ extern "C" int dvc_colorize_clip(dvc_ctx* c, const float* L_in, int F, int H, in
     c->err = first_err;
     return rc;
   }
-  if (!join_ok) return fail(c, DVC_ERR_CUDA, "colorize_clip: joining the internal streams failed");
-  if (se != cudaSuccess) return fail(c, DVC_ERR_CUDA, std::string("colorize_clip: ") + cudaGetErrorString(se));
+  if (!join_ok) return fail(c, DVC_ERR_CUDA, std::string(what) + ": joining the internal streams failed");
+  if (se != cudaSuccess) return fail(c, DVC_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(se));
   return DVC_OK;
+}
+
+extern "C" int dvc_colorize_clip(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature,
+                                 const float* first_last, float* ab_out, void* stream) {
+  return colorize_clip_impl(c, L_in, F, H, W, temperature, first_last, 0, ab_out, stream);
+}
+
+extern "C" int dvc_colorize_clip_exemplars(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature,
+                                           const float* first_last, int K, float* ab_out, void* stream) {
+  if (c && (K < 1 || K > 8)) return fail(c, DVC_ERR_ARG, "colorize_clip_exemplars: K must be in [1, 8]");
+  return colorize_clip_impl(c, L_in, F, H, W, temperature, first_last, K, ab_out, stream);
 }
 
 // ---- pre / post-processing around the nets (SURVEY.md §8f row 1) -----------------------------------------
@@ -1967,6 +2067,7 @@ extern "C" int64_t dvc_exemplar_pack_size(const dvc_ctx*, int H, int W) {
 extern "C" int dvc_exemplar_export(dvc_ctx* c, float* buf, int64_t n, void* stream) {
   if (!c || !buf) return c ? fail(c, DVC_ERR_ARG, "exemplar_export: bad argument") : DVC_ERR_ARG;
   if (!c->ex_valid) return fail(c, DVC_ERR_STATE, "exemplar_export: no exemplar set");
+  if (c->ex_K != 1) return fail(c, DVC_ERR_STATE, "exemplar_export: several exemplars are cached (dvc_set_exemplars); export packs one");
   const int64_t N = c->ex_N;
   if (n != N * 260) return fail(c, DVC_ERR_SHAPE, "exemplar_export: buffer size mismatch");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1982,20 +2083,13 @@ extern "C" int dvc_exemplar_import(dvc_ctx* c, const float* buf, int64_t n, int 
   if (n != N * 260) return fail(c, DVC_ERR_SHAPE, "exemplar_import: buffer size mismatch");
   cudaStream_t s = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->device));
-  if (c->ex_N != N) {
-    if (c->ex_phi) cudaFree(c->ex_phi);
-    if (c->ex_V) cudaFree(c->ex_V);
-    c->ex_phi = c->ex_V = nullptr;
-    CUDA_TRY(c, cudaMalloc((void**)&c->ex_phi, (size_t)N * 256 * 4));
-    CUDA_TRY(c, cudaMalloc((void**)&c->ex_V, (size_t)N * 16));
-    c->ex_N = (int)N;
-  }
+  DVC_TRY(ex_alloc(c, 1, (int)N));
   CUDA_TRY(c, cudaMemcpyAsync(c->ex_phi, buf, (size_t)N * 256 * 4, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(c, cudaMemcpyAsync(c->ex_V, buf + N * 256, (size_t)N * 16, cudaMemcpyDeviceToDevice, s));
   // whatever produced the pack, the 4th lane of every V row must be 1 (corr_tc.cu's softmax epilogue)
   launch_pack_v4(nullptr, c->ex_V, (size_t)N, s);
   DVC_TRY(check_launch(c, "pack_v4"));
-  c->ex_H = H, c->ex_W = W, c->ex_valid = true, c->ex_version++;
+  c->ex_H = H, c->ex_W = W, c->ex_K = 1, c->ex_valid = true, c->ex_version++;
   if (corr_ws_reserve(&c->corr_ws, 1, 1, (int)N, (int)N) != 0) return fail(c, DVC_ERR_CUDA, "exemplar_import: correlation workspace allocation failed");
   return DVC_OK;
 }

@@ -185,14 +185,15 @@ void launch_pack_v4(const float* src3, float* dst4, size_t n, cudaStream_t s);
 // y rows [B][N][4], sim rows [B][N] at h x w -> nearest x4 NCHW (NonlocalNet.py:499-500)
 void launch_rows_to_nchw_up4(const float* yrows, const float* simrows, float* y, float* sim, int B, int h, int w,
                              cudaStream_t s);
-// ColorVidNet input (FrameColor.py:64): [L, warped a, warped b, sim, last L, last a, last b, 0]
-void launch_build_color_input(const float* IA_l, const float* yrows, const float* simrows, const float* last_lab,
-                              float* dst, int B, int H, int W, int P, cudaStream_t s);
+// ColorVidNet input (FrameColor.py:64): [L, warped a, warped b, sim, last L, last a, last b, 0].  l_bstride: floats
+// between the L planes of consecutive batches (H * W, or 0: one luminance plane shared by every batch)
+void launch_build_color_input(const float* IA_l, size_t l_bstride, const float* yrows, const float* simrows,
+                              const float* last_lab, float* dst, int B, int H, int W, int P, cudaStream_t s);
 // conv10_ab (1x1, 128 -> 2) + tanh * 128 (ColorVidNet.py:143-144) -> NCHW [B][2][H][W]
 void launch_final_ab(const float* x, int H, int W, int P, int C, const float* w /*[2][C]*/, const float* bias,
                      float* out, int B, cudaStream_t s);
-// next frame's "last" = cat(L, ab) (test.py:96)
-void launch_make_last(const float* IA_l, const float* ab, float* last, int B, int H, int W, cudaStream_t s);
+// next frame's "last" = cat(L, ab) (test.py:96); l_bstride as for launch_build_color_input
+void launch_make_last(const float* IA_l, size_t l_bstride, const float* ab, float* last, int B, int H, int W, cudaStream_t s);
 
 // ---- correlation + softmax + warp (K7) ----------------------------------------------------------
 // Peer outputs of a query-row-sharded correlation (SURVEY.md 8e, config 4): the rank that owns query rows
@@ -206,10 +207,13 @@ struct CorrPeers {
 };
 
 struct CorrParams {
-  const float* theta;  // [B][NA][C]  (position-major, channels contiguous)
+  const float* theta;  // [B][NA][C]  (position-major, channels contiguous); [1][NA][C] when theta_shared
   const float* phi;    // [Bphi][NB][C]
   const float* V;      // [Bphi][NB][4] = (L, a, b, 1)
   int B, Bphi, NA, NB, C;
+  // one query set for every batch (query batch stride 0): batch b is that frame against reference set b (Bphi == B),
+  // e.g. one frame against K exemplars, without K copies of theta or of its operand planes
+  bool theta_shared = false;
   float temperature;
   float* y;     // [B][NA][4]
   float* sim;   // [B][NA]

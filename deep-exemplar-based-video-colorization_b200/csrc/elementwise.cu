@@ -470,7 +470,7 @@ __global__ void __launch_bounds__(256) rows_to_nchw_up4_kernel(const float* __re
   }
 }
 
-__global__ void __launch_bounds__(256) build_color_input_kernel(const float* __restrict__ IA_l,
+__global__ void __launch_bounds__(256) build_color_input_kernel(const float* __restrict__ IA_l, size_t l_bstride,
                                                                 const float* __restrict__ yrows,
                                                                 const float* __restrict__ simrows,
                                                                 const float* __restrict__ last, float* __restrict__ dst,
@@ -487,7 +487,7 @@ __global__ void __launch_bounds__(256) build_color_input_kernel(const float* __r
       const size_t q = (size_t)y * W + x;
       const int n = (y >> 2) * w + (x >> 2);
       const float4 yr = __ldg(reinterpret_cast<const float4*>(yrows + ((size_t)b * h * w + n) * 4));
-      o0.x = __ldg(IA_l + (size_t)b * plane + q);
+      o0.x = __ldg(IA_l + (size_t)b * l_bstride + q);
       o0.y = yr.y;  // warped a (channel 1 of the warped Lab, FrameColor.py:63)
       o0.z = yr.z;  // warped b
       o0.w = __ldg(simrows + (size_t)b * h * w + n);
@@ -534,11 +534,11 @@ __global__ void __launch_bounds__(256) final_ab_kernel(const float* __restrict__
   }
 }
 
-__global__ void __launch_bounds__(256) make_last_kernel(const float* __restrict__ IA_l, const float* __restrict__ ab,
-                                                        float* __restrict__ last, int HW) {
+__global__ void __launch_bounds__(256) make_last_kernel(const float* __restrict__ IA_l, size_t l_bstride,
+                                                        const float* __restrict__ ab, float* __restrict__ last, int HW) {
   const int b = blockIdx.y;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x) {
-    last[((size_t)b * 3 + 0) * HW + i] = IA_l[(size_t)b * HW + i];
+    last[((size_t)b * 3 + 0) * HW + i] = IA_l[(size_t)b * l_bstride + i];
     last[((size_t)b * 3 + 1) * HW + i] = ab[((size_t)b * 2 + 0) * HW + i];
     last[((size_t)b * 3 + 2) * HW + i] = ab[((size_t)b * 2 + 1) * HW + i];
   }
@@ -694,10 +694,10 @@ void launch_rows_to_nchw_up4(const float* yrows, const float* simrows, float* y,
   launch_counter_add(1);
 }
 
-void launch_build_color_input(const float* IA_l, const float* yrows, const float* simrows, const float* last_lab,
-                              float* dst, int B, int H, int W, int P, cudaStream_t s) {
+void launch_build_color_input(const float* IA_l, size_t l_bstride, const float* yrows, const float* simrows,
+                              const float* last_lab, float* dst, int B, int H, int W, int P, cudaStream_t s) {
   dim3 grid(grid_for((long)(H + 2 * P) * (W + 2 * P), 256), B);
-  build_color_input_kernel<<<grid, 256, 0, s>>>(IA_l, yrows, simrows, last_lab, dst, H, W, P);
+  build_color_input_kernel<<<grid, 256, 0, s>>>(IA_l, l_bstride, yrows, simrows, last_lab, dst, H, W, P);
   launch_counter_add(1);
 }
 
@@ -708,9 +708,9 @@ void launch_final_ab(const float* x, int H, int W, int P, int C, const float* w,
   launch_counter_add(1);
 }
 
-void launch_make_last(const float* IA_l, const float* ab, float* last, int B, int H, int W, cudaStream_t s) {
+void launch_make_last(const float* IA_l, size_t l_bstride, const float* ab, float* last, int B, int H, int W, cudaStream_t s) {
   dim3 grid(grid_for((long)H * W, 256), B);
-  make_last_kernel<<<grid, 256, 0, s>>>(IA_l, ab, last, H * W);
+  make_last_kernel<<<grid, 256, 0, s>>>(IA_l, l_bstride, ab, last, H * W);
   launch_counter_add(1);
 }
 

@@ -25,7 +25,8 @@ EXPORTED = [
     "dvc_resize_half", "dvc_upsample2_scaled", "dvc_lab_to_rgb8", "dvc_rgb8_to_lab",
     "dvc_fgs_filter", "dvc_l_to_guide8", "dvc_resize_antialias_crop_rgb8", "dvc_contextual_loss_forward",
     "dvc_peer_buffer_create", "dvc_peer_buffer_open", "dvc_peer_buffer_close", "dvc_peer_buffer_destroy",
-    "dvc_corr_set_peer_outputs",
+    "dvc_corr_set_peer_outputs", "dvc_set_exemplars", "dvc_colorize_frames_exemplars", "dvc_colorize_clip_exemplars",
+    "dvc_corr_softmax_warp_exemplars",
 ]
 
 _lib = None
@@ -67,6 +68,12 @@ def load_library():
         lib.dvc_colorize_frames.argtypes = [c_void, c_void, c_void, c_int, c_int, c_int, c_float, c_void, c_void, c_void,
                                             c_void]
         lib.dvc_colorize_clip.argtypes = [c_void, c_void, c_int, c_int, c_int, c_float, c_void, c_void, c_void]
+        lib.dvc_set_exemplars.argtypes = [c_void, c_void, c_int, c_int, c_int, c_void]
+        lib.dvc_colorize_frames_exemplars.argtypes = [c_void, c_void, c_void, c_int, c_int, c_int, c_float, c_void, c_void,
+                                                      c_void, c_void]
+        lib.dvc_colorize_clip_exemplars.argtypes = [c_void, c_void, c_int, c_int, c_int, c_float, c_void, c_int, c_void, c_void]
+        lib.dvc_corr_softmax_warp_exemplars.argtypes = [c_void, c_void, c_void, c_void, c_int, c_int, c_int, c_int, c_float,
+                                                        c_void, c_void, c_void, c_void]
         lib.dvc_exemplar_pack_size.argtypes = [c_void, c_int, c_int]
         lib.dvc_exemplar_pack_size.restype = c_i64
         lib.dvc_exemplar_export.argtypes = [c_void, c_void, c_i64, c_void]
@@ -130,6 +137,7 @@ class Context:
             raise DvcError(f"dvc_create failed ({rc}): {self.lib.dvc_last_error(None).decode()}")
         self.h = h
         self._weight_sig = {}
+        self.n_exemplars = 1  # exemplars cached by set_exemplar(s) / exemplar_import (sizes the *_exemplars outputs)
 
     def close(self):
         if getattr(self, "h", None):
@@ -229,6 +237,22 @@ class Context:
         self._check(rc, "dvc_corr_softmax_warp")
         return (y, sim, am) if want_argmax else (y, sim)
 
+    def corr_softmax_warp_exemplars(self, theta_hat, phi_hat, V, temperature, want_argmax=False):
+        """One query set theta_hat [1,C,NA] against K reference sets phi_hat [K,C,NB], V [K,NB,3] -> y [K,NA,3],
+        sim [K,NA] (, argmax [K,NA])."""
+        theta_hat, phi_hat, V = _dev_f32(theta_hat, "theta_hat"), _dev_f32(phi_hat, "phi_hat"), _dev_f32(V, "V")
+        _, C, NA = theta_hat.shape
+        K, _, NB = phi_hat.shape
+        if theta_hat.shape[0] != 1 or phi_hat.shape[1] != C or tuple(V.shape) != (K, NB, 3):
+            raise DvcError("corr_softmax_warp_exemplars: expected theta_hat [1,C,NA], phi_hat [K,C,NB], V [K,NB,3]")
+        y = torch.empty(K, NA, 3, device=theta_hat.device, dtype=torch.float32)
+        sim = torch.empty(K, NA, device=theta_hat.device, dtype=torch.float32)
+        am = torch.empty(K, NA, device=theta_hat.device, dtype=torch.int32) if want_argmax else None
+        rc = self.lib.dvc_corr_softmax_warp_exemplars(self.h, _ptr(theta_hat), _ptr(phi_hat), _ptr(V), K, NA, NB, C,
+                                                      float(temperature), _ptr(y), _ptr(sim), _ptr(am), _stream(theta_hat.device))
+        self._check(rc, "dvc_corr_softmax_warp_exemplars")
+        return (y, sim, am) if want_argmax else (y, sim)
+
     # ---- fused per-frame / per-clip path ---------------------------------------------------------
     def set_exemplar(self, IB_lab):
         t = IB_lab.detach().to(torch.float32).contiguous()
@@ -236,8 +260,62 @@ class Context:
             raise DvcError("exemplar must be [1,3,H,W]")
         self._check(self.lib.dvc_set_exemplar(self.h, _ptr(t), t.shape[2], t.shape[3], _stream(self.device)),
                     "dvc_set_exemplar")
+        self.n_exemplars = 1
         if not t.is_cuda:
             torch.cuda.current_stream(self.device).synchronize()  # the host buffer must outlive the async copy
+
+    def set_exemplars(self, IB_lab):
+        """K exemplars [K,3,H,W] (test.py:168-181 runs the clip once per reference image): each gets set_exemplar's
+        prologue into a slot of its own; colorize_frames_exemplars / colorize_clip_exemplars then run against all K."""
+        t = IB_lab.detach().to(torch.float32).contiguous()
+        if t.dim() != 4 or t.shape[1] != 3:
+            raise DvcError("exemplars must be [K,3,H,W]")
+        self._check(self.lib.dvc_set_exemplars(self.h, _ptr(t), t.shape[0], t.shape[2], t.shape[3], _stream(self.device)),
+                    "dvc_set_exemplars")
+        self.n_exemplars = t.shape[0]
+        if not t.is_cuda:
+            torch.cuda.current_stream(self.device).synchronize()
+
+    def colorize_frames_exemplars(self, IA_l, last, temperature=1e-10, want_warp=False):
+        """One frame IA_l [1,1,H,W] against the K cached exemplars, last [K,3,H,W] -> ab [K,2,H,W]
+        (, warp [K,3,H,W], sim [K,1,H,W])."""
+        IA_l, last = _dev_f32(IA_l, "IA_l"), _dev_f32(last, "last")
+        _, c1, H, W = IA_l.shape
+        K = last.shape[0]
+        if IA_l.shape[0] != 1 or c1 != 1 or tuple(last.shape[1:]) != (3, H, W):
+            raise DvcError("colorize_frames_exemplars: IA_l must be [1,1,H,W] and last [K,3,H,W]")
+        ab = torch.empty(K, 2, H, W, device=IA_l.device, dtype=torch.float32)
+        warp = torch.empty(K, 3, H, W, device=IA_l.device, dtype=torch.float32) if want_warp else None
+        sim = torch.empty(K, 1, H, W, device=IA_l.device, dtype=torch.float32) if want_warp else None
+        rc = self.lib.dvc_colorize_frames_exemplars(self.h, _ptr(IA_l), _ptr(last), K, H, W, float(temperature), _ptr(ab),
+                                                    _ptr(warp), _ptr(sim), _stream(IA_l.device))
+        self._check(rc, "dvc_colorize_frames_exemplars")
+        return (ab, warp, sim) if want_warp else ab
+
+    def colorize_clip_exemplars(self, L, temperature=1e-10, first_last_lab=None, out=None):
+        """L [F,1,H,W] -> ab [K,F,2,H,W]: colorize_clip against each of the K cached exemplars (K independent recurrences,
+        test.py:76-96), with the exemplar-independent half of every frame computed once.  first_last_lab: None (zeros) or
+        [K,3,H,W].  L pinned on the host or on the device; `out` lives where L lives."""
+        if L.dtype != torch.float32 or L.dim() != 4 or L.shape[1] != 1:
+            raise DvcError("colorize_clip_exemplars takes a float32 [F,1,H,W] tensor")
+        L = L.contiguous()
+        F_, _, H, W = L.shape
+        K = self.n_exemplars
+        if out is None:
+            out = torch.empty(K, F_, 2, H, W, dtype=torch.float32, device=L.device)
+            if not L.is_cuda:
+                out = out.pin_memory()
+        if out.is_cuda != L.is_cuda or not out.is_contiguous() or tuple(out.shape) != (K, F_, 2, H, W):
+            raise DvcError("colorize_clip_exemplars: `out` must be a contiguous [K,F,2,H,W] tensor on the same side as L")
+        fl = None
+        if first_last_lab is not None:
+            fl = first_last_lab.to(torch.float32).contiguous()
+            if tuple(fl.shape) != (K, 3, H, W):
+                raise DvcError("colorize_clip_exemplars: first_last_lab must be [K,3,H,W]")
+        rc = self.lib.dvc_colorize_clip_exemplars(self.h, _ptr(L), F_, H, W, float(temperature), _ptr(fl), K, _ptr(out),
+                                                  _stream(self.device))
+        self._check(rc, "dvc_colorize_clip_exemplars")
+        return out
 
     def colorize_frames(self, IA_l, IA_last_lab, temperature=1e-10, want_warp=False):
         IA_l, IA_last_lab = _dev_f32(IA_l, "IA_l"), _dev_f32(IA_last_lab, "IA_last_lab")
@@ -410,6 +488,7 @@ class Context:
         buf = _dev_f32(buf, "exemplar pack")
         self._check(self.lib.dvc_exemplar_import(self.h, _ptr(buf), buf.numel(), H, W, _stream(self.device)),
                     "dvc_exemplar_import")
+        self.n_exemplars = 1
 
     # ---- debug hooks ---------------------------------------------------------------------------------
     def debug_flag(self, name, value):

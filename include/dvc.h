@@ -103,6 +103,13 @@ int dvc_colorvidnet_forward(dvc_ctx* ctx, const float* dev_x, int B, int H, int 
 int dvc_corr_softmax_warp(dvc_ctx* ctx, const float* dev_theta_hat, const float* dev_phi_hat,
                           const float* dev_V, int B, int Bphi, int NA, int NB, int C, float temperature,
                           float* dev_y, float* dev_sim, int32_t* dev_argmax, void* stream);
+/* One query set against K reference sets (1 <= K <= 8; the correlation of dvc_colorize_frames_exemplars): theta_hat
+ * [1,C,NA], phi_hat [K,C,NB], V [K,NB,3] -> y [K,NA,3], sim [K,NA], argmax [K,NA] (may be NULL).  Slot k equals
+ * dvc_corr_softmax_warp(theta_hat, phi_hat[k], V[k]) except for the summation order of softmax weights (T > 0) and of
+ * the V rows of bit-equal maxima.  Not combined with peer outputs (dvc_corr_set_peer_outputs): DVC_ERR_STATE. */
+int dvc_corr_softmax_warp_exemplars(dvc_ctx* ctx, const float* dev_theta_hat, const float* dev_phi_hat, const float* dev_V,
+                                    int K, int NA, int NB, int C, float temperature, float* dev_y, float* dev_sim,
+                                    int32_t* dev_argmax, void* stream);
 
 /* ---- fused per-frame / per-clip path (test.py:57-96 + FrameColor.py:41-67) -------------------- */
 
@@ -123,6 +130,29 @@ int dvc_colorize_frames(dvc_ctx* ctx, const float* dev_IA_l, const float* dev_IA
  * host [1,3,H,W] tensor (test.py:78, --frame_propagate).  Synchronises `stream` before returning. */
 int dvc_colorize_clip(dvc_ctx* ctx, const float* host_L, int F, int H, int W, float temperature,
                       const float* host_first_last_lab, float* host_ab, void* stream);
+
+/* ---- several exemplars for one clip (test.py:168-181 colorizes the clip once per reference image) ------------
+ * The half of every frame that does not depend on the exemplar (VGG19, feature_normalize, the WarpNet query side)
+ * runs once; the correlation runs against all K cached exemplars and ColorVidNet at batch K.  Exemplar k's results
+ * are those of frame_colorization(IA_t, IB_k, last_k) with last_k = cat(L_t, ab_k,t-1) (test.py:96): K independent
+ * recurrences sharing one luminance sequence.  While K > 1 exemplars are cached, dvc_colorize_frames,
+ * dvc_colorize_clip and dvc_exemplar_export return DVC_ERR_STATE; dvc_set_exemplar / dvc_exemplar_import cache one
+ * again.  K outside [1, 8] is DVC_ERR_ARG, a K other than the cached count or a frame size other than the
+ * exemplars' is DVC_ERR_SHAPE. */
+
+/* K exemplars IB_lab [K,3,H,W] (host or device pointer): dvc_set_exemplar's prologue for each, cached in K slots (slot
+ * k holds exactly what dvc_set_exemplar(IB_k) caches).  dvc_set_exemplar / dvc_exemplar_import are the K = 1 case. */
+int dvc_set_exemplars(dvc_ctx* ctx, const float* IB_lab, int K, int H, int W, void* stream);
+/* One frame against all K cached exemplars.  dev_IA_l [1,1,H,W]; dev_last_lab [K,3,H,W]; dev_out_ab [K,2,H,W];
+ * optional dev_out_warp_lab [K,3,H,W] and dev_out_sim [K,1,H,W] (may be NULL).  K must equal the cached count. */
+int dvc_colorize_frames_exemplars(dvc_ctx* ctx, const float* dev_IA_l, const float* dev_last_lab, int K, int H, int W,
+                                  float temperature, float* dev_out_ab, float* dev_out_warp_lab, float* dev_out_sim,
+                                  void* stream);
+/* dvc_colorize_clip with K recurrences: L [F,1,H,W]; first_last_lab NULL (zeros, test.py:80) or [K,3,H,W]
+ * (--frame_propagate, test.py:78); ab [K,F,2,H,W], so each exemplar's clip is contiguous.  Host (pinned) or device
+ * memory, like dvc_colorize_clip.  Synchronises `stream` before returning. */
+int dvc_colorize_clip_exemplars(dvc_ctx* ctx, const float* L, int F, int H, int W, float temperature,
+                                const float* first_last_lab, int K, float* ab, void* stream);
 
 /* ---- pre / post-processing around the nets (SURVEY.md §8f row 1) ------------------------------ */
 
