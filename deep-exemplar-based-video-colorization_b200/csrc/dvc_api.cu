@@ -12,6 +12,7 @@
 #include <cstring>
 #include <map>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -164,6 +165,10 @@ struct dvc_ctx {
   cudaEvent_t evA[4] = {nullptr, nullptr, nullptr, nullptr}, evC[4] = {nullptr, nullptr, nullptr, nullptr}, evFork = nullptr,
               evJoinA = nullptr, evJoinC = nullptr, evJoinD = nullptr;
   cudaEvent_t evU[4] = {nullptr, nullptr, nullptr, nullptr}, evD[4] = {nullptr, nullptr, nullptr, nullptr};
+  // video driver (dvc_colorize_video_rgb8): the clip's streams plus frame ingest and post-processing
+  cudaStream_t sI = nullptr, sP = nullptr;
+  cudaEvent_t evR[4] = {nullptr, nullptr, nullptr, nullptr}, evP[4] = {nullptr, nullptr, nullptr, nullptr};
+  cudaEvent_t evJoinI = nullptr, evJoinP = nullptr;
   // exemplar cache: ex_K slots (dvc_set_exemplars; 1 after dvc_set_exemplar / dvc_exemplar_import), room for ex_slots
   float* ex_phi = nullptr;  // [K][N][256]
   float* ex_V = nullptr;    // [K][N][4]
@@ -1140,6 +1145,14 @@ extern "C" int dvc_destroy(dvc_ctx* c) {
   if (c->evJoinD) cudaEventDestroy(c->evJoinD);
   if (c->sU) cudaStreamDestroy(c->sU);
   if (c->sD) cudaStreamDestroy(c->sD);
+  if (c->sI) cudaStreamDestroy(c->sI);
+  if (c->sP) cudaStreamDestroy(c->sP);
+  for (int i = 0; i < 4; ++i) {
+    if (c->evR[i]) cudaEventDestroy(c->evR[i]);
+    if (c->evP[i]) cudaEventDestroy(c->evP[i]);
+  }
+  if (c->evJoinI) cudaEventDestroy(c->evJoinI);
+  if (c->evJoinP) cudaEventDestroy(c->evJoinP);
   if (c->ex_phi) cudaFree(c->ex_phi);
   if (c->ex_V) cudaFree(c->ex_V);
   corr_ws_free(&c->corr_ws);
@@ -1776,6 +1789,169 @@ static int clip_streams(dvc_ctx* c) {
   return DVC_OK;
 }
 
+// ---- host-side constants of the pre / post-processing kernels ---------------------------------------------------------
+static void gaussian_taps(double sigma, std::vector<double>* w, int* radius) {  // scipy.ndimage._gaussian_kernel1d, truncate = 4
+  const int r = (int)(4.0 * sigma + 0.5);
+  w->assign(2 * r + 1, 0.0);
+  const double s2 = sigma * sigma;
+  double sum = 0.0;
+  for (int x = -r; x <= r; ++x) (*w)[x + r] = exp(-0.5 / s2 * (double)(x * x)), sum += (*w)[x + r];
+  for (double& v : *w) v /= sum;
+  *radius = r;
+}
+
+// CenterPad's anti-aliasing filter, skimage.transform.resize: sigma = max(0, (in / out - 1) / 2) per axis, applied axis 0
+// first (scipy.ndimage.gaussian_filter).  An axis that needs no filter gets no taps (radius 0).
+static void resize_taps(int Hs, int Ws, int Hr, int Wr, std::vector<double>* wy, int* ry, std::vector<double>* wx, int* rx) {
+  const double sy = fmax(0.0, ((double)Hs / Hr - 1.0) / 2.0), sx = fmax(0.0, ((double)Ws / Wr - 1.0) / 2.0);
+  wy->clear(), wx->clear();
+  *ry = *rx = 0;
+  if (sy > 1e-15) gaussian_taps(sy, wy, ry);
+  if (sx > 1e-15) gaussian_taps(sx, wx, rx);
+}
+
+// FGS weights_LUT[d] = -exp(-d / sigma_color), d = |difference of neighbouring guide pixels|: evaluated in double and
+// rounded once to the fp32 work type (the oracle does the same, so the two agree bit for bit)
+static void fgs_lut(float sigma_color, float lut[256]) {
+  for (int d = 0; d < 256; ++d) lut[d] = (float)(-exp(-(double)d / (double)sigma_color));
+}
+
+// num_iter FGS iterations (a horizontal and a vertical sweep each) over `planes` planes in place, lambda attenuated per iteration
+static void fgs_sweeps(float* planes_data, const float* Ch, const float* Cv, float* D, int planes, int H, int W, float lambda,
+                       float lambda_attenuation, int num_iter, cudaStream_t s) {
+  float lam = lambda;
+  for (int n = 0; n < num_iter; ++n) {
+    launch_fgs_horizontal(planes_data, Ch, D, planes, H, W, lam, s);
+    launch_fgs_vertical(planes_data, Cv, D, planes, H, W, lam, s);
+    lam *= lambda_attenuation;
+  }
+}
+
+// rgb_from_xyz = inv(xyz_from_rgb) (skimage.color.colorconv), by the adjugate in double precision
+static void rgb_from_xyz(double inv[9]) {
+  const double a[9] = {0.412453, 0.357580, 0.180423, 0.212671, 0.715160, 0.072169, 0.019334, 0.119193, 0.950227};
+  const double det = a[0] * (a[4] * a[8] - a[5] * a[7]) - a[1] * (a[3] * a[8] - a[5] * a[6]) + a[2] * (a[3] * a[7] - a[4] * a[6]);
+  const double m[9] = {(a[4] * a[8] - a[5] * a[7]) / det, (a[2] * a[7] - a[1] * a[8]) / det, (a[1] * a[5] - a[2] * a[4]) / det,
+                       (a[5] * a[6] - a[3] * a[8]) / det, (a[0] * a[8] - a[2] * a[6]) / det, (a[2] * a[3] - a[0] * a[5]) / det,
+                       (a[3] * a[7] - a[4] * a[6]) / det, (a[1] * a[6] - a[0] * a[7]) / det, (a[0] * a[4] - a[1] * a[3]) / det};
+  for (int i = 0; i < 9; ++i) inv[i] = m[i];
+}
+
+// ---- dvc_colorize_video_rgb8: frame ingest and post-processing around the clip loop --------------------------------------
+// Ring slots (frame t uses slot t & 1 or t & 3) guarded by events of the frame that last used the slot; the kernels of one
+// stage run in order on one stream, so the stage's scratch buffers (fp64 resize planes, crop, FGS Ch / Cv / D, up-sampled
+// ab) exist once.  Nothing depends on F.
+struct VideoIO {
+  const unsigned char* frames = nullptr;  // [F][Hs][Ws][3], host (pinned) or device
+  int Hs = 0, Ws = 0, Hr = 0, Wr = 0, oy = 0, ox = 0, Ho = 0, Wo = 0;
+  bool wls = false;
+  float lambda = 0.f, sigma = 0.f;
+  unsigned char* out = nullptr;  // [K][F][Ho][Wo][3], host (pinned) or device
+  float* last_out = nullptr;     // [K][3][Ho/2][Wo/2] or nullptr
+  std::vector<double> taps;      // [wy | wx | 1.0]: uploaded once per call
+  int ry = 0, rx = 0, ny = 0, nx = 0;
+  float lut[256];
+  // device workspaces
+  unsigned char *src = nullptr, *crop = nullptr, *guide = nullptr, *rgb = nullptr;
+  double *f0 = nullptr, *f1 = nullptr, *dtaps = nullptr;
+  float *dlut = nullptr, *L = nullptr, *abL = nullptr, *Ch = nullptr, *Cv = nullptr, *D = nullptr;
+};
+
+static int video_streams(dvc_ctx* c) {
+  if (c->sI) return DVC_OK;
+  CUDA_TRY(c, cudaStreamCreateWithFlags(&c->sI, cudaStreamNonBlocking));
+  CUDA_TRY(c, cudaStreamCreateWithFlags(&c->sP, cudaStreamNonBlocking));
+  for (int i = 0; i < 4; ++i) {
+    CUDA_TRY(c, cudaEventCreateWithFlags(&c->evR[i], cudaEventDisableTiming));
+    CUDA_TRY(c, cudaEventCreateWithFlags(&c->evP[i], cudaEventDisableTiming));
+  }
+  CUDA_TRY(c, cudaEventCreateWithFlags(&c->evJoinI, cudaEventDisableTiming));
+  CUDA_TRY(c, cudaEventCreateWithFlags(&c->evJoinP, cudaEventDisableTiming));
+  return DVC_OK;
+}
+
+// workspaces, then the taps and the LUT on `s` (before the clip loop forks from it)
+static int video_prologue(dvc_ctx* c, VideoIO& v, int Kb, cudaStream_t s) {
+  const size_t ns = (size_t)v.Hs * v.Ws * 3, hw = (size_t)v.Ho * v.Wo;
+  auto raw = [&](const char* name, size_t bytes, auto** out) {
+    void* p = nullptr;
+    const int rc = get_raw(c, name, bytes, &p, s);
+    *out = (std::remove_pointer_t<decltype(out)>)p;
+    return rc;
+  };
+  DVC_TRY(raw("vid.src", 2 * ns, &v.src));  // 2 slots
+  DVC_TRY(raw("vid.f0", ns * 8, &v.f0));
+  DVC_TRY(raw("vid.f1", ns * 8, &v.f1));
+  DVC_TRY(raw("vid.taps", v.taps.size() * 8, &v.dtaps));
+  DVC_TRY(raw("vid.crop", hw * 3, &v.crop));
+  DVC_TRY(raw("vid.L", 4 * hw * 4, &v.L));  // 4 slots, like the half-resolution L of the clip loop
+  DVC_TRY(raw("vid.abL", (size_t)Kb * 2 * hw * 4, &v.abL));
+  DVC_TRY(raw("vid.rgb", 2 * (size_t)Kb * hw * 3, &v.rgb));  // 2 slots
+  if (v.wls) {
+    DVC_TRY(raw("vid.guide", 4 * hw, &v.guide));  // 4 slots
+    DVC_TRY(raw("vid.lut", 256 * 4, &v.dlut));
+    DVC_TRY(raw("vid.Ch", hw * 4, &v.Ch));
+    DVC_TRY(raw("vid.Cv", hw * 4, &v.Cv));
+    DVC_TRY(raw("vid.D", (size_t)Kb * 2 * hw * 4, &v.D));
+    CUDA_TRY(c, cudaMemcpyAsync(v.dlut, v.lut, sizeof(v.lut), cudaMemcpyHostToDevice, s));
+  }
+  CUDA_TRY(c, cudaMemcpyAsync(v.dtaps, v.taps.data(), v.taps.size() * 8, cudaMemcpyHostToDevice, s));
+  return DVC_OK;
+}
+
+// frame t: upload (stream U) -> CenterPad resize -> L, L/2 (into the clip loop's slot Lt) and the guide (stream I);
+// records evU[t & 3], which phase A waits for
+static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
+  const size_t ns = (size_t)v.Hs * v.Ws * 3, hw = (size_t)v.Ho * v.Wo;
+  unsigned char* src = v.src + (size_t)(t & 1) * ns;
+  // the source slot was last read by frame t-2's resize
+  if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sU, c->evU[(t - 2) & 3], 0));
+  CUDA_TRY(c, cudaMemcpyAsync(src, v.frames + (size_t)t * ns, ns, cudaMemcpyDefault, c->sU));
+  CUDA_TRY(c, cudaEventRecord(c->evR[t & 3], c->sU));
+  // the half-resolution L slot was last read by frame t-4's ColorVidNet / make_last, the full-resolution L and guide slots
+  // by frame t-4's post-processing
+  CUDA_TRY(c, cudaStreamWaitEvent(c->sI, c->evR[t & 3], 0));
+  if (t >= 4) CUDA_TRY(c, cudaStreamWaitEvent(c->sI, c->evC[(t - 4) & 3], 0));
+  if (t >= 4) CUDA_TRY(c, cudaStreamWaitEvent(c->sI, c->evP[(t - 4) & 3], 0));
+  // dvc_resize_antialias_crop_rgb8's kernel sequence; a zero-radius "filter" (one tap of weight 1) converts uint8 -> float64
+  double *cur = v.f0, *nxt = v.f1;
+  launch_gauss_axis_u8(src, cur, v.ny ? v.dtaps : v.dtaps + v.ny + v.nx, v.ry, 1, v.Hs, v.Ws * 3, c->sI);
+  if (v.nx) {
+    launch_gauss_axis_f64(cur, nxt, v.dtaps + v.ny, v.rx, (size_t)v.Hs, v.Ws, 3, c->sI);
+    std::swap(cur, nxt);
+  }
+  launch_zoom_crop(cur, v.Hs, v.Ws, v.Hr, v.Wr, v.oy, v.ox, v.crop, v.Ho, v.Wo, c->sI);
+  launch_rgb8_to_l_half(v.crop, v.L + (size_t)(t & 3) * hw, Lt, v.wls ? v.guide + (size_t)(t & 3) * hw : nullptr, v.Ho, v.Wo, c->sI);
+  DVC_TRY(check_launch(c, "video ingest"));
+  CUDA_TRY(c, cudaEventRecord(c->evU[t & 3], c->sI));
+  return DVC_OK;
+}
+
+// frame t, once its ColorVidNet is done (evC[t & 3]): ab x2 * 1.25, FGS, Lab -> sRGB (stream P; records evP[t & 3], which
+// the reuse of the ab slot waits for) and the download (stream D; records evD[t & 3])
+static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int Kb, int F) {
+  const size_t hw = (size_t)v.Ho * v.Wo;
+  unsigned char* rgb = v.rgb + (size_t)(t & 1) * Kb * hw * 3;
+  CUDA_TRY(c, cudaStreamWaitEvent(c->sP, c->evC[t & 3], 0));
+  if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sP, c->evD[(t - 2) & 3], 0));  // the rgb slot has been downloaded
+  launch_upsample2(abt, v.abL, Kb * 2, v.Ho / 2, v.Wo / 2, 1.25f, c->sP);  // test.py:100-102
+  if (v.wls) {  // test.py:105-112: the a and b planes of every exemplar against the frame's one guide
+    launch_fgs_weights(v.guide + (size_t)(t & 3) * hw, v.dlut, v.Ch, v.Cv, v.Ho, v.Wo, c->sP);
+    fgs_sweeps(v.abL, v.Ch, v.Cv, v.D, Kb * 2, v.Ho, v.Wo, v.lambda, 0.25f, 3, c->sP);
+  }
+  double inv[9];
+  rgb_from_xyz(inv);
+  for (int k = 0; k < Kb; ++k)  // test.py:116-119, the frame's full-resolution L for every exemplar
+    launch_lab_to_rgb8(v.L + (size_t)(t & 3) * hw, v.abL + (size_t)k * 2 * hw, rgb + (size_t)k * hw * 3, 1, v.Ho, v.Wo, inv, c->sP);
+  DVC_TRY(check_launch(c, "video post-processing"));
+  CUDA_TRY(c, cudaEventRecord(c->evP[t & 3], c->sP));
+  CUDA_TRY(c, cudaStreamWaitEvent(c->sD, c->evP[t & 3], 0));
+  for (int k = 0; k < Kb; ++k)
+    CUDA_TRY(c, cudaMemcpyAsync(v.out + ((size_t)k * F + t) * hw * 3, rgb + (size_t)k * hw * 3, hw * 3, cudaMemcpyDefault, c->sD));
+  CUDA_TRY(c, cudaEventRecord(c->evD[t & 3], c->sD));
+  return DVC_OK;
+}
+
 // test.py:68-96 for one contiguous segment.  Frame t+1's frame-independent phase (VGG / WarpNet / correlation)
 // runs on stream A while frame t's ColorVidNet -- which needs frame t-1's prediction -- runs on stream C; the
 // partial waves of either leave SMs idle that the other fills.  Uploads of L (up to four frames ahead) and downloads
@@ -1784,10 +1960,12 @@ static int clip_streams(dvc_ctx* c) {
 // K = 0: dvc_colorize_clip (one exemplar); K >= 1: dvc_colorize_clip_exemplars, K recurrences sharing the luminance
 // sequence -- phase A once per frame against the K slots, phase C at batch K, and ab of exemplar k, frame t at
 // ab_out + (k F + t) 2 H W.  The multi-exemplar workspaces have tags of their own, so alternating does not reallocate.
+// v != nullptr (dvc_colorize_video_rgb8): frame t's L comes from video_ingest instead of L_in, and video_post replaces the
+// download of ab; the recurrence state after the last frame goes to v->last_out.
 static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature, const float* first_last,
-                              int K, float* ab_out, void* stream) {
-  const char* what = K ? "colorize_clip_exemplars" : "colorize_clip";
-  if (!c || !L_in || !ab_out || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
+                              int K, float* ab_out, void* stream, VideoIO* v = nullptr) {
+  const char* what = v ? "colorize_video_rgb8" : (K ? "colorize_clip_exemplars" : "colorize_clip");
+  if (!c || (!v && (!L_in || !ab_out)) || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
   if (K < 0 || K > 8) return fail(c, DVC_ERR_ARG, std::string(what) + ": K must be in [1, 8]");
   DVC_TRY(check_frame_args(c, H, W, temperature, K));
   const int Kb = K ? K : 1;  // batch of phase C
@@ -1795,6 +1973,7 @@ static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W
   cudaStream_t s = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->device));
   DVC_TRY(clip_streams(c));
+  if (v) DVC_TRY(video_streams(c));
   const size_t hw = (size_t)H * W;
   const int N = (H / 4) * (W / 4);
   void *dL, *dlast, *dab, *yrows, *simrows;
@@ -1806,6 +1985,7 @@ static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W
   const bool two_a = c->clip_astreams == 2;
   // the second phase-A stream has its own correlation workspace (sized like the first at dvc_set_exemplar time)
   if (two_a && corr_ws_reserve(&c->corr_ws2, Kb, Kb, N, N) != 0) return fail(c, DVC_ERR_CUDA, std::string(what) + ": correlation workspace allocation failed");
+  if (v) DVC_TRY(video_prologue(c, *v, Kb, s));
   if (first_last)
     CUDA_TRY(c, cudaMemcpyAsync(dlast, first_last, Kb * 3 * hw * 4, cudaMemcpyDefault, s));
   else
@@ -1819,6 +1999,10 @@ static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W
     CUDA_TRY(c, cudaStreamWaitEvent(c->sC, c->evFork, 0));
     CUDA_TRY(c, cudaStreamWaitEvent(c->sU, c->evFork, 0));
     CUDA_TRY(c, cudaStreamWaitEvent(c->sD, c->evFork, 0));
+    if (v) {
+      CUDA_TRY(c, cudaStreamWaitEvent(c->sI, c->evFork, 0));
+      CUDA_TRY(c, cudaStreamWaitEvent(c->sP, c->evFork, 0));
+    }
     for (int t = 0; t < F; ++t) {
       const int slot = t & 1;
       float* Lt = (float*)dL + (size_t)(t & 3) * hw;
@@ -1827,10 +2011,14 @@ static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W
       float* sr = (float*)simrows + (size_t)(t & 3) * Kb * N;
       const bool odd = two_a && (t & 1);
       cudaStream_t sAt = odd ? c->sA2 : c->sA;
-      // ---- upload stream: the L slot was last read by frame t-4's ColorVidNet / make_last ----
-      if (t >= 4) CUDA_TRY(c, cudaStreamWaitEvent(c->sU, c->evC[(t - 4) & 3], 0));
-      CUDA_TRY(c, cudaMemcpyAsync(Lt, L_in + (size_t)t * hw, hw * 4, cudaMemcpyDefault, c->sU));
-      CUDA_TRY(c, cudaEventRecord(c->evU[t & 3], c->sU));
+      if (v) {
+        DVC_TRY(video_ingest(c, *v, t, Lt));
+      } else {
+        // ---- upload stream: the L slot was last read by frame t-4's ColorVidNet / make_last ----
+        if (t >= 4) CUDA_TRY(c, cudaStreamWaitEvent(c->sU, c->evC[(t - 4) & 3], 0));
+        CUDA_TRY(c, cudaMemcpyAsync(Lt, L_in + (size_t)t * hw, hw * 4, cudaMemcpyDefault, c->sU));
+        CUDA_TRY(c, cudaEventRecord(c->evU[t & 3], c->sU));
+      }
       // ---- stream A (two of them, alternating, when clip_astreams = 2): the frame-independent phase; the reuse of the
       // warp-row slot waits for frame t-4's ColorVidNet ----
       CUDA_TRY(c, cudaStreamWaitEvent(sAt, c->evU[t & 3], 0));
@@ -1840,17 +2028,24 @@ static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W
       CUDA_TRY(c, cudaEventRecord(c->evA[t & 3], sAt));
       // ---- stream C: the recurrent phase (the K recurrences read the frame's one L plane) ----
       CUDA_TRY(c, cudaStreamWaitEvent(c->sC, c->evA[t & 3], 0));
-      if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sC, c->evD[(t - 2) & 3], 0));  // the ab slot has been downloaded
+      // the ab slot has been downloaded (video: post-processed)
+      if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sC, (v ? c->evP : c->evD)[(t - 2) & 3], 0));
       DVC_TRY(frames_phaseC(c, K ? "clipCx" : "clipC", Lt, yr, sr, (float*)dlast, Kb, H, W, abt, c->sC, 0));
       launch_make_last(Lt, 0, abt, (float*)dlast, Kb, H, W, c->sC);  // test.py:96
       DVC_TRY(check_launch(c, "make_last"));
       CUDA_TRY(c, cudaEventRecord(c->evC[t & 3], c->sC));
+      if (v) {
+        DVC_TRY(video_post(c, *v, t, abt, Kb, F));
+        continue;
+      }
       // ---- download stream ----
       CUDA_TRY(c, cudaStreamWaitEvent(c->sD, c->evC[t & 3], 0));
       for (int k = 0; k < Kb; ++k)
         CUDA_TRY(c, cudaMemcpyAsync(ab_out + ((size_t)k * F + t) * 2 * hw, abt + (size_t)k * 2 * hw, 2 * hw * 4, cudaMemcpyDefault, c->sD));
       CUDA_TRY(c, cudaEventRecord(c->evD[t & 3], c->sD));
     }
+    if (v && v->last_out)  // cat(L/2, ab) of the last frame: the next segment's first_last
+      CUDA_TRY(c, cudaMemcpyAsync(v->last_out, dlast, Kb * 3 * hw * 4, cudaMemcpyDefault, c->sC));
     return DVC_OK;
   };
   const int rc = enqueue();
@@ -1862,11 +2057,16 @@ static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W
   join_ok &= cudaEventRecord(c->evJoinC, c->sC) == cudaSuccess && cudaStreamWaitEvent(s, c->evJoinC, 0) == cudaSuccess;
   join_ok &= cudaEventRecord(c->evJoinD, c->sD) == cudaSuccess && cudaStreamWaitEvent(s, c->evJoinD, 0) == cudaSuccess;
   join_ok &= cudaEventRecord(c->evFork, c->sU) == cudaSuccess && cudaStreamWaitEvent(s, c->evFork, 0) == cudaSuccess;
+  if (v) {
+    join_ok &= cudaEventRecord(c->evJoinI, c->sI) == cudaSuccess && cudaStreamWaitEvent(s, c->evJoinI, 0) == cudaSuccess;
+    join_ok &= cudaEventRecord(c->evJoinP, c->sP) == cudaSuccess && cudaStreamWaitEvent(s, c->evJoinP, 0) == cudaSuccess;
+  }
   const cudaError_t se = cudaStreamSynchronize(s);
   if (rc != DVC_OK) {
     if (!join_ok || se != cudaSuccess) {  // could not even drain the streams: make sure nothing is in flight
       cudaStreamSynchronize(c->sA), cudaStreamSynchronize(c->sA2), cudaStreamSynchronize(c->sC), cudaStreamSynchronize(c->sU),
           cudaStreamSynchronize(c->sD);
+      if (v) cudaStreamSynchronize(c->sI), cudaStreamSynchronize(c->sP);
     }
     c->err = first_err;
     return rc;
@@ -1885,6 +2085,34 @@ extern "C" int dvc_colorize_clip_exemplars(dvc_ctx* c, const float* L_in, int F,
                                            const float* first_last, int K, float* ab_out, void* stream) {
   if (c && (K < 1 || K > 8)) return fail(c, DVC_ERR_ARG, "colorize_clip_exemplars: K must be in [1, 8]");
   return colorize_clip_impl(c, L_in, F, H, W, temperature, first_last, K, ab_out, stream);
+}
+
+// test.py:68-120 end to end: ingest, the clip loop and the post-processing of every frame in one pipeline (see VideoIO)
+extern "C" int dvc_colorize_video_rgb8(dvc_ctx* c, const unsigned char* frames, int F, int Hs, int Ws, int Hr, int Wr, int oy, int ox,
+                                       int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda,
+                                       float wls_sigma, unsigned char* out, float* last_lab_out, void* stream) {
+  const char* what = "colorize_video_rgb8";
+  if (!c || !frames || !out || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
+  if (Hs < 1 || Ws < 1 || Hr < 1 || Wr < 1 || Ho < 2 || Wo < 2 || (Ho & 1) || (Wo & 1))
+    return fail(c, DVC_ERR_SHAPE, std::string(what) + ": bad geometry (sizes >= 1, an even output size)");
+  // the output window and the resized image nest in one another along each axis: a crop of it, or a zero pad around it
+  auto nested = [](int resized, int outsz, int off) { return resized >= outsz ? off >= 0 && off <= resized - outsz : off <= 0 && off >= resized - outsz; };
+  if (!nested(Hr, Ho, oy) || !nested(Wr, Wo, ox)) return fail(c, DVC_ERR_SHAPE, std::string(what) + ": crop offset outside the resized image");
+  DVC_TRY(check_frame_shape(c, what, Ho / 2, Wo / 2));
+  if (wls && !(wls_lambda >= 0.f && wls_sigma > 0.f)) return fail(c, DVC_ERR_ARG, std::string(what) + ": bad WLS parameter");
+  VideoIO v;
+  v.frames = frames, v.Hs = Hs, v.Ws = Ws, v.Hr = Hr, v.Wr = Wr, v.oy = oy, v.ox = ox, v.Ho = Ho, v.Wo = Wo;
+  v.wls = wls != 0, v.lambda = wls_lambda, v.sigma = wls_sigma, v.out = out, v.last_out = last_lab_out;
+  std::vector<double> wy, wx;
+  resize_taps(Hs, Ws, Hr, Wr, &wy, &v.ry, &wx, &v.rx);
+  v.ny = (int)wy.size(), v.nx = (int)wx.size();
+  v.taps = wy;
+  v.taps.insert(v.taps.end(), wx.begin(), wx.end());
+  v.taps.push_back(1.0);
+  if (v.wls) fgs_lut(wls_sigma, v.lut);
+  // one exemplar: the single-exemplar loop (and its workspaces), as dvc_colorize_clip
+  const int K = c->ex_valid && c->ex_K > 1 ? c->ex_K : 0;
+  return colorize_clip_impl(c, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, K, nullptr, stream, &v);
 }
 
 // ---- pre / post-processing around the nets (SURVEY.md §8f row 1) -----------------------------------------
@@ -1908,12 +2136,8 @@ extern "C" int dvc_lab_to_rgb8(dvc_ctx* c, const float* dev_l, const float* dev_
                                void* stream) {
   if (!c || !dev_l || !dev_ab || !dev_rgb || B < 1 || H < 1 || W < 1) return c ? fail(c, DVC_ERR_ARG, "lab_to_rgb8: bad argument") : DVC_ERR_ARG;
   CUDA_TRY(c, cudaSetDevice(c->device));
-  // rgb_from_xyz = inv(xyz_from_rgb) (skimage.color.colorconv), by the adjugate in double precision
-  const double a[9] = {0.412453, 0.357580, 0.180423, 0.212671, 0.715160, 0.072169, 0.019334, 0.119193, 0.950227};
-  const double det = a[0] * (a[4] * a[8] - a[5] * a[7]) - a[1] * (a[3] * a[8] - a[5] * a[6]) + a[2] * (a[3] * a[7] - a[4] * a[6]);
-  const double inv[9] = {(a[4] * a[8] - a[5] * a[7]) / det, (a[2] * a[7] - a[1] * a[8]) / det, (a[1] * a[5] - a[2] * a[4]) / det,
-                         (a[5] * a[6] - a[3] * a[8]) / det, (a[0] * a[8] - a[2] * a[6]) / det, (a[2] * a[3] - a[0] * a[5]) / det,
-                         (a[3] * a[7] - a[4] * a[6]) / det, (a[1] * a[6] - a[0] * a[7]) / det, (a[0] * a[4] - a[1] * a[3]) / det};
+  double inv[9];
+  rgb_from_xyz(inv);
   launch_lab_to_rgb8(dev_l, dev_ab, dev_rgb, B, H, W, inv, (cudaStream_t)stream);
   return check_launch(c, "lab_to_rgb8");
 }
@@ -1982,21 +2206,14 @@ extern "C" int dvc_fgs_filter(dvc_ctx* c, const unsigned char* dev_guide, const 
   DVC_TRY(get_raw(c, "fgs.Ch", hw * 4, &Ch, s));
   DVC_TRY(get_raw(c, "fgs.Cv", hw * 4, &Cv, s));
   DVC_TRY(get_raw(c, "fgs.D", (size_t)planes * hw * 4, &D, s));
-  // weights_LUT[d] = -exp(-d / sigma_color), d = |difference of neighbouring guide pixels|: evaluated in double and
-  // rounded once to the fp32 work type (the oracle does the same, so the two agree bit for bit)
   float h_lut[256];
-  for (int d = 0; d < 256; ++d) h_lut[d] = (float)(-exp(-(double)d / (double)sigma_color));
+  fgs_lut(sigma_color, h_lut);
   CUDA_TRY(c, cudaMemcpyAsync(lut, h_lut, sizeof(h_lut), cudaMemcpyHostToDevice, s));
   CUDA_TRY(c, cudaStreamSynchronize(s));  // h_lut lives on this stack frame
   launch_fgs_weights(dev_guide, (const float*)lut, (float*)Ch, (float*)Cv, H, W, s);
   DVC_TRY(check_launch(c, "fgs_weights"));
   if (dev_dst != dev_src) CUDA_TRY(c, cudaMemcpyAsync(dev_dst, dev_src, (size_t)planes * hw * 4, cudaMemcpyDeviceToDevice, s));
-  float lam = lambda;
-  for (int n = 0; n < num_iter; ++n) {
-    launch_fgs_horizontal(dev_dst, (const float*)Ch, (float*)D, planes, H, W, lam, s);
-    launch_fgs_vertical(dev_dst, (const float*)Cv, (float*)D, planes, H, W, lam, s);
-    lam *= lambda_attenuation;
-  }
+  fgs_sweeps(dev_dst, (const float*)Ch, (const float*)Cv, (float*)D, planes, H, W, lambda, lambda_attenuation, num_iter, s);
   return check_launch(c, "fgs");
 }
 
@@ -2008,16 +2225,6 @@ extern "C" int dvc_l_to_guide8(dvc_ctx* c, const float* dev_l, int H, int W, uns
 }
 
 // ---- CenterPad's anti-aliased resize + crop / pad (util_distortion.py:217-258) ---------------------------------------
-static void gaussian_taps(double sigma, std::vector<double>* w, int* radius) {  // scipy.ndimage._gaussian_kernel1d, truncate = 4
-  const int r = (int)(4.0 * sigma + 0.5);
-  w->assign(2 * r + 1, 0.0);
-  const double s2 = sigma * sigma;
-  double sum = 0.0;
-  for (int x = -r; x <= r; ++x) (*w)[x + r] = exp(-0.5 / s2 * (double)(x * x)), sum += (*w)[x + r];
-  for (double& v : *w) v /= sum;
-  *radius = r;
-}
-
 extern "C" int dvc_resize_antialias_crop_rgb8(dvc_ctx* c, const unsigned char* dev_src, int Hs, int Ws, int Hr, int Wr, int oy, int ox,
                                               unsigned char* dev_dst, int Ho, int Wo, void* stream) {
   if (!c || !dev_src || !dev_dst || Hs < 1 || Ws < 1 || Hr < 1 || Wr < 1 || Ho < 1 || Wo < 1)
@@ -2029,12 +2236,9 @@ extern "C" int dvc_resize_antialias_crop_rgb8(dvc_ctx* c, const unsigned char* d
   DVC_TRY(get_raw(c, "rs.f0", n * 8, &f0, s));
   DVC_TRY(get_raw(c, "rs.f1", n * 8, &f1, s));
   DVC_TRY(get_raw(c, "rs.taps", 8192 * 8, &taps, s));
-  // skimage.transform.resize: sigma = max(0, (in / out - 1) / 2) per axis, applied axis 0 first (scipy.ndimage.gaussian_filter)
-  const double sy = fmax(0.0, ((double)Hs / Hr - 1.0) / 2.0), sx = fmax(0.0, ((double)Ws / Wr - 1.0) / 2.0);
   std::vector<double> wy, wx;
   int ry = 0, rx = 0;
-  if (sy > 1e-15) gaussian_taps(sy, &wy, &ry);
-  if (sx > 1e-15) gaussian_taps(sx, &wx, &rx);
+  resize_taps(Hs, Ws, Hr, Wr, &wy, &ry, &wx, &rx);
   if (wy.size() + wx.size() > 8192) return fail(c, DVC_ERR_SHAPE, "resize_antialias_crop: down-scaling factor too large");
   if (!wy.empty()) CUDA_TRY(c, cudaMemcpyAsync(taps, wy.data(), wy.size() * 8, cudaMemcpyHostToDevice, s));
   if (!wx.empty()) CUDA_TRY(c, cudaMemcpyAsync((double*)taps + wy.size(), wx.data(), wx.size() * 8, cudaMemcpyHostToDevice, s));

@@ -69,6 +69,28 @@ __device__ __forceinline__ void block_amax_commit(float amax, ScaleCell* cell, f
     if (m > 0.f) atomicMax(&cell->amax_bits, __float_as_uint(m));
   }
 }
+// util_distortion.py:18-23 -> skimage.color.rgb2lab of one uint8 pixel in float64: f(X/Xn), f(Y/Yn), f(Z/Zn).  Shared by
+// rgb8_to_lab_kernel and the fused video ingest, which must give bit-identical L.
+__device__ __forceinline__ void rgb8_lab_f(const unsigned char* __restrict__ px, double f[3]) {
+  double c[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const double v = (double)px[k] / 255.0;
+    c[k] = v > 0.04045 ? pow((v + 0.055) / 1.055, 2.4) : v / 12.92;
+  }
+  const double M[9] = {0.412453, 0.357580, 0.180423, 0.212671, 0.715160, 0.072169, 0.019334, 0.119193, 0.950227};
+  const double white[3] = {0.95047, 1.0, 1.08883};
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const double t = (c[0] * M[k * 3 + 0] + c[1] * M[k * 3 + 1] + c[2] * M[k * 3 + 2]) / white[k];
+    f[k] = t > 0.008856 ? cbrt(t) : 7.787 * t + 16.0 / 116.0;
+  }
+}
+// test.py:106: the WLS guide uint8(uncenter_l(L) * 255 / 100) of a centred L value, fp32, truncation toward zero
+__device__ __forceinline__ unsigned char guide8_of_l(float l) {
+  const float v = __fdiv_rn(__fmul_rn(__fadd_rn(l, 50.f), 255.f), 100.f);
+  return (unsigned char)fminf(fmaxf(truncf(v), 0.f), 255.f);
+}
 #endif
 
 struct Act {
@@ -248,6 +270,9 @@ void launch_fgs_weights(const unsigned char* guide, const float* lut, float* Ch,
 void launch_fgs_horizontal(float* cur, const float* Ch, float* D, int planes, int H, int W, float lam, cudaStream_t s);
 void launch_fgs_vertical(float* cur, const float* Cv, float* D, int planes, int H, int W, float lam, cudaStream_t s);
 void launch_l_to_guide8(const float* l, unsigned char* g, size_t n, cudaStream_t s);
+// video ingest: uint8 [H][W][3] (H, W even) -> centred L [H][W] (rgb8_to_lab's plane 0), its 1/2 resolution [H/2][W/2]
+// (resize_half of that plane) and, when guide != nullptr, the WLS guide [H][W] (l_to_guide8 of the L plane)
+void launch_rgb8_to_l_half(const unsigned char* rgb, float* l, float* l_half, unsigned char* guide, int H, int W, cudaStream_t s);
 void launch_gauss_axis_u8(const unsigned char* src, double* dst, const double* w, int radius, size_t n_outer, int len, int inner,
                           cudaStream_t s);
 void launch_gauss_axis_f64(const double* src, double* dst, const double* w, int radius, size_t n_outer, int len, int inner,

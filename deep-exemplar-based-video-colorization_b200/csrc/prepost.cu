@@ -130,9 +130,35 @@ __global__ void __launch_bounds__(32) fgs_horizontal_kernel(float* __restrict__ 
 
 // test.py:106: guide = uint8(uncenter_l(L) * 255 / 100), fp32 arithmetic, truncation toward zero
 __global__ void __launch_bounds__(256) l_to_guide8_kernel(const float* __restrict__ l, unsigned char* __restrict__ g, size_t n) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float v = __fdiv_rn(__fmul_rn(__fadd_rn(__ldg(l + i), 50.f), 255.f), 100.f);
-    g[i] = (unsigned char)fminf(fmaxf(truncf(v), 0.f), 255.f);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    g[i] = guide8_of_l(__ldg(l + i));
+}
+
+// Video ingest (test.py:44-46,71,106 for the luminance only -- the frames' a / b are never used).  A warp owns a 2 x 16
+// pixel tile (lane = row * 16 + column) of the centred uint8 frame, one thread per pixel; the 2 x 2 neighbourhoods of the
+// half-resolution plane are gathered with shuffles.  L is rgb8_to_lab_kernel's plane 0 (the same float64 operations,
+// rgb8_lab_f), the half-resolution value resize_half_kernel's arithmetic on those four floats, the guide l_to_guide8's.
+__global__ void __launch_bounds__(256) rgb8_to_l_half_kernel(const unsigned char* __restrict__ rgb, float* __restrict__ l,
+                                                             float* __restrict__ l_half, unsigned char* __restrict__ guide, int H,
+                                                             int W) {
+  const int lane = threadIdx.x & 31;
+  const int tw = (W + 15) / 16, ntiles = (H / 2) * tw, nwarps = gridDim.x * (blockDim.x >> 5);
+  for (int tile = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); tile < ntiles; tile += nwarps) {  // warp-uniform
+    const int i = tile / tw, x = (tile - i * tw) * 16 + (lane & 15), y = 2 * i + (lane >> 4);
+    float v = 0.f;
+    if (x < W) {
+      const size_t pix = (size_t)y * W + x;
+      double f[3];
+      rgb8_lab_f(rgb + pix * 3, f);
+      v = (float)(116.0 * f[1] - 16.0) - 50.0f;
+      l[pix] = v;
+      if (guide) guide[pix] = guide8_of_l(v);
+    }
+    // resize_half: 0.5 * (0.5 * a.x + 0.5 * a.y) + 0.5 * (0.5 * b.x + 0.5 * b.y), a = row 2i, b = row 2i + 1
+    const float nb = __shfl_xor_sync(0xffffffffu, v, 1);
+    const float r = (lane & 1) ? 0.5f * nb + 0.5f * v : 0.5f * v + 0.5f * nb;
+    const float r1 = __shfl_xor_sync(0xffffffffu, r, 16);
+    if (lane < 16 && !(lane & 1) && x < W) l_half[(size_t)i * (W / 2) + x / 2] = 0.5f * r + 0.5f * r1;
   }
 }
 
@@ -318,6 +344,10 @@ void launch_fgs_vertical(float* cur, const float* Cv, float* D, int planes, int 
 }
 void launch_l_to_guide8(const float* l, unsigned char* g, size_t n, cudaStream_t s) {
   l_to_guide8_kernel<<<grid_for(n, 256), 256, 0, s>>>(l, g, n);
+  launch_counter_add(1);
+}
+void launch_rgb8_to_l_half(const unsigned char* rgb, float* l, float* l_half, unsigned char* guide, int H, int W, cudaStream_t s) {
+  rgb8_to_l_half_kernel<<<grid_for((size_t)(H / 2) * ((W + 15) / 16) * 32, 256), 256, 0, s>>>(rgb, l, l_half, guide, H, W);
   launch_counter_add(1);
 }
 void launch_gauss_axis_u8(const unsigned char* src, double* dst, const double* w, int radius, size_t n_outer, int len, int inner,

@@ -26,7 +26,7 @@ EXPORTED = [
     "dvc_fgs_filter", "dvc_l_to_guide8", "dvc_resize_antialias_crop_rgb8", "dvc_contextual_loss_forward",
     "dvc_peer_buffer_create", "dvc_peer_buffer_open", "dvc_peer_buffer_close", "dvc_peer_buffer_destroy",
     "dvc_corr_set_peer_outputs", "dvc_set_exemplars", "dvc_colorize_frames_exemplars", "dvc_colorize_clip_exemplars",
-    "dvc_corr_softmax_warp_exemplars",
+    "dvc_corr_softmax_warp_exemplars", "dvc_colorize_video_rgb8",
 ]
 
 _lib = None
@@ -74,6 +74,8 @@ def load_library():
         lib.dvc_colorize_clip_exemplars.argtypes = [c_void, c_void, c_int, c_int, c_int, c_float, c_void, c_int, c_void, c_void]
         lib.dvc_corr_softmax_warp_exemplars.argtypes = [c_void, c_void, c_void, c_void, c_int, c_int, c_int, c_int, c_float,
                                                         c_void, c_void, c_void, c_void]
+        lib.dvc_colorize_video_rgb8.argtypes = [c_void, c_void, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                                c_float, c_void, c_int, c_float, c_float, c_void, c_void, c_void]
         lib.dvc_exemplar_pack_size.argtypes = [c_void, c_int, c_int]
         lib.dvc_exemplar_pack_size.restype = c_i64
         lib.dvc_exemplar_export.argtypes = [c_void, c_void, c_i64, c_void]
@@ -350,6 +352,50 @@ class Context:
                                         _stream(self.device))
         self._check(rc, "dvc_colorize_clip")
         return out
+
+    def colorize_video_rgb8(self, frames, size, temperature=1e-10, first_last_lab=None, wls=(500.0, 4.0), out=None,
+                            return_last=False):
+        """test.py:68-120 end to end: uint8 frames [F,Hs,Ws,3] -> sRGB uint8 [K,F,size[0],size[1],3], one image per cached
+        exemplar and frame.  Per frame: CenterPad + CenterCrop to `size`, Lab, 1/2, the networks (colorize_clip's
+        recurrence), ab x2 * 1.25, the WLS filter (wls = (lambda, sigma_color), or None to skip it) and Lab -> sRGB, all
+        in one pipelined call whose device memory does not grow with F.
+
+        frames: pinned CPU or CUDA (a pageable CPU tensor is pinned first); `out` lives where frames live.
+        first_last_lab: None (zeros, test.py:80) or [K,3,size[0]/2,size[1]/2].  return_last=True also returns the
+        recurrence state after the last frame, cat(L, ab) at half resolution [K,3,size[0]/2,size[1]/2] on the same side
+        as frames: passed as the next call's first_last_lab it continues the clip exactly (chunked streaming)."""
+        from dvc.prepost import centerpad_geometry
+
+        if not (isinstance(frames, torch.Tensor) and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3):
+            raise DvcError("colorize_video_rgb8: expected a uint8 tensor [F,Hs,Ws,3]")
+        frames = frames.contiguous()
+        if not frames.is_cuda and not frames.is_pinned():
+            frames = frames.pin_memory()
+        F_, Hs, Ws, _ = frames.shape
+        Ho, Wo = int(size[0]), int(size[1])
+        Hr, Wr, oy, ox = centerpad_geometry(Hs, Ws, (Ho, Wo))
+        K = self.n_exemplars
+
+        def host_or_device(shape, dtype):
+            t = torch.empty(*shape, dtype=dtype, device=frames.device)
+            return t if frames.is_cuda else t.pin_memory()
+
+        if out is None:
+            out = host_or_device((K, F_, Ho, Wo, 3), torch.uint8)
+        if (out.is_cuda != frames.is_cuda or out.dtype != torch.uint8 or not out.is_contiguous()
+                or tuple(out.shape) != (K, F_, Ho, Wo, 3)):
+            raise DvcError("colorize_video_rgb8: `out` must be a contiguous uint8 [K,F,H,W,3] tensor on the same side as frames")
+        fl = None
+        if first_last_lab is not None:
+            fl = first_last_lab.to(torch.float32).contiguous()
+            if tuple(fl.shape) != (K, 3, Ho // 2, Wo // 2):
+                raise DvcError("colorize_video_rgb8: first_last_lab must be [K,3,H/2,W/2]")
+        last = host_or_device((K, 3, Ho // 2, Wo // 2), torch.float32) if return_last else None
+        lam, sigma = (0.0, 1.0) if wls is None else (float(wls[0]), float(wls[1]))
+        rc = self.lib.dvc_colorize_video_rgb8(self.h, _ptr(frames), F_, Hs, Ws, Hr, Wr, oy, ox, Ho, Wo, float(temperature), _ptr(fl),
+                                              0 if wls is None else 1, lam, sigma, _ptr(out), _ptr(last), _stream(self.device))
+        self._check(rc, "dvc_colorize_video_rgb8")
+        return (out, last) if return_last else out
 
     # ---- pre / post-processing around the nets (test.py:58,71,100-102) ----------------------------------
     def resize_half(self, x):

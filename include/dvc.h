@@ -153,6 +153,22 @@ int dvc_colorize_frames_exemplars(dvc_ctx* ctx, const float* dev_IA_l, const flo
  * memory, like dvc_colorize_clip.  Synchronises `stream` before returning. */
 int dvc_colorize_clip_exemplars(dvc_ctx* ctx, const float* L, int F, int H, int W, float temperature,
                                 const float* first_last_lab, int K, float* ab, void* stream);
+/* test.py:68-120 end to end on the device, in one pipelined call: per frame of frames [F,Hs,Ws,3] (uint8 sRGB)
+ *   CenterPad + CenterCrop (dvc_resize_antialias_crop_rgb8 with the geometry Hr, Wr, oy, ox, Ho, Wo, which the caller
+ *   computes: dvc/prepost.py) -> centred L at Ho x Wo and at (Ho/2) x (Wo/2) (dvc_rgb8_to_lab's plane 0, dvc_resize_half;
+ *   the frames' a / b are not computed) -> the networks against the K cached exemplars (dvc_colorize_clip /
+ *   dvc_colorize_clip_exemplars; K = 1 after dvc_set_exemplar) -> ab x2 * 1.25 (dvc_upsample2_scaled) -> if wls, the
+ *   Fast Global Smoother (wls_lambda, wls_sigma; lambda_attenuation 0.25, 3 iterations) of every a / b plane guided by
+ *   dvc_l_to_guide8 of the full-resolution L -> dvc_lab_to_rgb8 with that L
+ * into out [K,F,Ho,Wo,3] uint8.  The cached exemplar size must be (Ho/2, Wo/2); the output window must nest with the
+ * resized image (0 <= oy <= Hr - Ho, or Hr - Ho <= oy <= 0; the same for x).  first_last_lab: NULL (zeros) or
+ * [K,3,Ho/2,Wo/2]; last_lab_out: NULL or [K,3,Ho/2,Wo/2], receives cat(L/2, ab) of the last frame, so a clip cut into
+ * segments, each continuing from the previous one's last_lab_out, gives the bytes of one call over the whole clip.
+ * frames / out / first_last_lab / last_lab_out may be host (pinned) or device memory.  Device memory does not depend on
+ * F.  Synchronises `stream` before returning; a refused call launches nothing. */
+int dvc_colorize_video_rgb8(dvc_ctx* ctx, const unsigned char* frames, int F, int Hs, int Ws, int Hr, int Wr, int oy, int ox,
+                            int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda,
+                            float wls_sigma, unsigned char* out, float* last_lab_out, void* stream);
 
 /* ---- pre / post-processing around the nets (SURVEY.md §8f row 1) ------------------------------ */
 
