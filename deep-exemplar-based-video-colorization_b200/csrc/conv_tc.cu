@@ -1,4 +1,5 @@
-// Convolution on the Hopper tensor cores (wgmma + TMA + mbarrier): DVC_MATH_TF32X3 (and its 3xFP16 default).
+// Convolution on the Hopper tensor cores (wgmma + TMA + mbarrier): DVC_MATH_TF32X3 (and its 3xFP16 default), and the
+// one-pass DVC_MATH_FP16X1 (see P1 below).
 //
 // Same flat shifted GEMM as conv_simt.cu (Y[p, co] = sum_tap sum_ci X[p + off(tap), ci] W[tap][ci][co] over the
 // padded pixel index p), with fp32-class accuracy from three 16/19-bit MMAs per product on hi/lo split operands
@@ -51,12 +52,14 @@ struct Geo {
 
 // KBY = bytes of K per pipeline stage and operand row: 128 (SWIZZLE_128B, 32 tf32 / 64 fp16) or 64 (SWIZZLE_64B).
 // Every CTA holds the whole weight tile of a stage (in a cluster half of it arrives by the peer's multicast).
-template <int BN, int KBY>
+// P1 (one pass): a stage holds the hi planes only, so the same shared memory holds twice as many stages.
+template <int BN, int KBY, bool P1 = false>
 struct Cfg {
-  static constexpr int STAGES = (BN == 256 ? 2 : (BN == 128 ? 3 : 4)) * (128 / KBY);
+  static constexpr int PLANES = P1 ? 1 : 2;
+  static constexpr int STAGES = (BN == 256 ? 2 : (BN == 128 ? 3 : 4)) * (128 / KBY) * (P1 ? 2 : 1);
   static constexpr int A_BYTES = Geo<BN>::BMT * KBY;
   static constexpr int B_BYTES = BN * KBY;
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
+  static constexpr int STAGE_BYTES = PLANES * A_BYTES + PLANES * B_BYTES;
   // + barriers + statistics [8 consumer warps][2][BN]
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 512 + 8 * 2 * BN * 4;
 };
@@ -66,15 +69,16 @@ struct Cfg {
 // activation tile of AR = BMT + 8 rows is loaded per (tap row, k-block) and the wgmma descriptors of the taps start dil *
 // 128 bytes apart: a third of the activation bytes through TMA and L2 (the weights still arrive per tap, in a ring of
 // their own).
-template <int BN>
+template <int BN, bool P1 = false>
 struct CfgRS {
+  static constexpr int PLANES = P1 ? 1 : 2;
   static constexpr int AR = Geo<BN>::BMT + 8;
   static constexpr int A_TILE = AR * 128;              // one plane (a multiple of the 1024-byte swizzle atom)
-  static constexpr int A_STAGE = 2 * A_TILE;           // hi + lo
+  static constexpr int A_STAGE = PLANES * A_TILE;      // hi + lo (P1: hi)
   static constexpr int B_TILE = BN * 128;
-  static constexpr int B_STAGE = 2 * B_TILE;
-  static constexpr int A_STAGES = (BN == 256) ? 2 : 3;
-  static constexpr int B_STAGES = (BN == 64) ? 4 : (BN == 128 ? 3 : 2);
+  static constexpr int B_STAGE = PLANES * B_TILE;
+  static constexpr int A_STAGES = ((BN == 256) ? 2 : 3) * (P1 ? 2 : 1);
+  static constexpr int B_STAGES = ((BN == 64) ? 4 : (BN == 128 ? 3 : 2)) * (P1 ? 2 : 1);
   static constexpr int RING_BYTES = A_STAGES * A_STAGE + B_STAGES * B_STAGE;
   static constexpr int SMEM_BYTES = RING_BYTES + 1024 + 512 + 8 * 2 * BN * 4;
 };
@@ -91,13 +95,17 @@ __device__ __forceinline__ float tf32_rna(float x) {
 // F16: operands are fp16 hi/lo planes of x * 2^e (e static per tensor / layer, chosen from a proven bound so that
 // nothing overflows): the same 2 x 11 significant bits as the tf32 split at twice the MMA rate, half the operand
 // bytes and half as many truncating accumulations per unit of K; the epilogue multiplies by 2^-(e_x + e_w) (exact).
-template <int BN, int CL, int KBY, bool F16, bool RS = false>
+// P1 (DVC_MATH_FP16X1): one MMA per product, hi.hi, on the same planes -- the producer loads X_hi and W_hi only and
+// the consumers issue one wgmma per k-step.  The operands are rounded to 11 significant bits (fp16 planes: the power-of-
+// two scale is exact; tf32 planes: cvt.rna), as cuDNN rounds fp32 convolution operands to TF32; the products are
+// exact and the accumulation is the three-pass engine's, so only the operand rounding differs from it.
+template <int BN, int CL, int KBY, bool F16, bool RS = false, bool P1 = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
     conv_tc_kernel(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUtensorMap tmXl,
                    const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const ConvTcParams p) {
   using G = Geo<BN>;
-  using C = Cfg<BN, KBY>;
-  using RC = CfgRS<BN>;
+  using C = Cfg<BN, KBY, P1>;
+  using RC = CfgRS<BN, P1>;
   static_assert(!RS || KBY == 128, "row-shared taps use 128-byte K blocks");
   constexpr int BMT = G::BMT, R = G::R;
   constexpr int A_BYTES = C::A_BYTES;
@@ -124,7 +132,10 @@ __global__ void __launch_bounds__(NTHREADS, 1)
   const int nk = p.taps * kbs;
   // Each wgmma accumulation truncates; a chunk of `kc` k-blocks (12*kc accumulations) is therefore summed in the
   // accumulator registers from zero and then added -- with round-to-nearest fp32 adds -- to a register total (the
-  // tensor-core analogue of conv_simt.cu's two-level accumulation).
+  // tensor-core analogue of conv_simt.cu's two-level accumulation).  Per 128-byte k-block the three-pass engine makes
+  // 12 accumulations of which 4 (hi.hi) are full-size; the one-pass engine makes those 4 only.  Either way a chunk
+  // holds 4*kc full-size truncating accumulations, so P1 keeps the chunk length and spends its halved stage size on
+  // twice the ring stages.
   const int kc = p.kc * (128 / KBY);  // p.kc counts 128-byte k-blocks
   const int nchunks = (nk + kc - 1) / kc;
   // Split-K against wave quantisation: a work item is (tile, split s of S); split s sums the chunks
@@ -138,9 +149,11 @@ __global__ void __launch_bounds__(NTHREADS, 1)
 
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tmXh);
-    tc::tma_prefetch_desc(&tmXl);
     tc::tma_prefetch_desc(&tmWh);
-    tc::tma_prefetch_desc(&tmWl);
+    if (!P1) {
+      tc::tma_prefetch_desc(&tmXl);
+      tc::tma_prefetch_desc(&tmWl);
+    }
     for (int i = 0; i < NFULL; ++i) tc::mbar_init(&full[i], 1), tc::mbar_init(&empty[i], 8 * CL);  // consumer warps of the cluster
     tc::fence_barrier_init();
   }
@@ -157,11 +170,11 @@ __global__ void __launch_bounds__(NTHREADS, 1)
       auto load_w = [&](uint8_t* st, uint64_t* fb, int kb, int wrow, int bbytes) {
         if (CL == 1) {
           tc::tma_load_2d(st, &tmWh, fb, kb * KE, wrow);
-          tc::tma_load_2d(st + bbytes, &tmWl, fb, kb * KE, wrow);
+          if (!P1) tc::tma_load_2d(st + bbytes, &tmWl, fb, kb * KE, wrow);
         } else {  // my half of the channel rows, multicast into both CTAs
           const int h = crank * (BN / 2);
           tc::tma_load_2d_mc(st + h * KBY, &tmWh, fb, kb * KE, wrow + h, 3);
-          tc::tma_load_2d_mc(st + bbytes + h * KBY, &tmWl, fb, kb * KE, wrow + h, 3);
+          if (!P1) tc::tma_load_2d_mc(st + bbytes + h * KBY, &tmWl, fb, kb * KE, wrow + h, 3);
         }
       };
       if constexpr (RS) {
@@ -182,7 +195,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
               const int row = m0 + p.tap_off[ty * ntx];
               tc::mbar_arrive_expect_tx(&full[as], RC::A_STAGE);
               tc::tma_load_2d(st, &tmXh, &full[as], kb * KE, row);
-              tc::tma_load_2d(st + RC::A_TILE, &tmXl, &full[as], kb * KE, row);
+              if (!P1) tc::tma_load_2d(st + RC::A_TILE, &tmXl, &full[as], kb * KE, row);
             }
             __syncwarp();
             if (++as == RC::A_STAGES) as = 0, aph ^= 1;
@@ -213,11 +226,11 @@ __global__ void __launch_bounds__(NTHREADS, 1)
             tc::mbar_wait(&empty[stage], phase ^ 1);
             if (tc::elect_one()) {
               uint8_t* st = smem + stage * C::STAGE_BYTES;
-              const bool skip_lo = (p.dbg & 2) != 0;  // TIMING EXPERIMENT ONLY (wrong results): do not fetch the activation lo plane
-              tc::mbar_arrive_expect_tx(&full[stage], C::STAGE_BYTES - (skip_lo ? A_BYTES : 0));
+              const bool skip_lo = P1 || (p.dbg & 2) != 0;  // dbg & 2: TIMING EXPERIMENT ONLY (wrong results): do not fetch the activation lo plane
+              tc::mbar_arrive_expect_tx(&full[stage], C::STAGE_BYTES - (skip_lo && !P1 ? A_BYTES : 0));
               tc::tma_load_2d(st, &tmXh, &full[stage], kb * KE, m0 + off);
               if (!skip_lo) tc::tma_load_2d(st + A_BYTES, &tmXl, &full[stage], kb * KE, m0 + off);
-              load_w(st + 2 * A_BYTES, &full[stage], kb, tap * p.CoutPad + n0, C::B_BYTES);
+              load_w(st + C::PLANES * A_BYTES, &full[stage], kb, tap * p.CoutPad + n0, C::B_BYTES);
             }
             __syncwarp();
             if (++stage == C::STAGES) stage = 0, phase ^= 1;
@@ -458,7 +471,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
       } else {
         tc::mbar_wait(&full[stage], phase);
         sa = tc::smem_u32(smem + stage * C::STAGE_BYTES) + (uint32_t)ro * KBY;
-        sb = tc::smem_u32(smem + stage * C::STAGE_BYTES + 2 * A_BYTES) + (uint32_t)co * KBY;
+        sb = tc::smem_u32(smem + stage * C::STAGE_BYTES + C::PLANES * A_BYTES) + (uint32_t)co * KBY;
       }
       constexpr uint32_t A_PLANE = RS ? RC::A_TILE : A_BYTES, B_PLANE = RS ? RC::B_TILE : C::B_BYTES;
       auto mkdesc = [](uint32_t x) { return KBY == 128 ? tc::wg_desc_k128(x) : tc::wg_desc_k64(x); };
@@ -466,19 +479,27 @@ __global__ void __launch_bounds__(NTHREADS, 1)
       const uint64_t dWh = mkdesc(sb), dWl = mkdesc(sb + B_PLANE);
       tc::wg_fence_regs(a);
       tc::wg_fence();
-      // Every accumulation truncates the accumulator at ITS current magnitude, so the two small cross terms of the
-      // whole k-block go first (while a fresh accumulator is still ~2^-11 of its final size, their truncations are
-      // negligible) and the dominant hi*hi terms last: 4 instead of 12 full-size truncations per k-block.
+      if constexpr (P1) {
 #pragma unroll
-      for (int kk = 0; kk < KBY / 32; ++kk) {
-        const uint64_t adv = (uint64_t)(kk * 2);
-        tc::wgmma_fmt<FMT>(a, dXl + adv, dWh + adv, (first && kk == 0) ? 0u : 1u);
-        tc::wgmma_fmt<FMT>(a, dXh + adv, dWl + adv, 1u);
-      }
+        for (int kk = 0; kk < KBY / 32; ++kk) {
+          const uint64_t adv = (uint64_t)(kk * 2);
+          tc::wgmma_fmt<FMT>(a, dXh + adv, dWh + adv, (first && kk == 0) ? 0u : 1u);
+        }
+      } else {
+        // Every accumulation truncates the accumulator at ITS current magnitude, so the two small cross terms of the
+        // whole k-block go first (while a fresh accumulator is still ~2^-11 of its final size, their truncations are
+        // negligible) and the dominant hi*hi terms last: 4 instead of 12 full-size truncations per k-block.
 #pragma unroll
-      for (int kk = 0; kk < KBY / 32; ++kk) {
-        const uint64_t adv = (uint64_t)(kk * 2);
-        tc::wgmma_fmt<FMT>(a, dXh + adv, dWh + adv, 1u);
+        for (int kk = 0; kk < KBY / 32; ++kk) {
+          const uint64_t adv = (uint64_t)(kk * 2);
+          tc::wgmma_fmt<FMT>(a, dXl + adv, dWh + adv, (first && kk == 0) ? 0u : 1u);
+          tc::wgmma_fmt<FMT>(a, dXh + adv, dWl + adv, 1u);
+        }
+#pragma unroll
+        for (int kk = 0; kk < KBY / 32; ++kk) {
+          const uint64_t adv = (uint64_t)(kk * 2);
+          tc::wgmma_fmt<FMT>(a, dXh + adv, dWh + adv, 1u);
+        }
       }
       tc::wg_commit();
       tc::wg_wait<1>();  // unconditional (a no-op without an older group), so ptxas sees every older group retired
@@ -540,13 +561,13 @@ __global__ void __launch_bounds__(NTHREADS, 1)
   if (CL == 2) tc::cluster_sync_all();  // no CTA may exit while its peer can still multicast into it or arrive on its barriers
 }
 
-template <int BN, int CL, int KBY, bool F16, bool RS = false>
+template <int BN, int CL, int KBY, bool F16, bool RS = false, bool P1 = false>
 int launch_bn(const CUtensorMap& mXh, const CUtensorMap& mXl, const CUtensorMap& mWh, const CUtensorMap& mWl,
               const ConvTcParams& p, int num_sms, cudaStream_t s) {
-  constexpr int SMEM = RS ? CfgRS<BN>::SMEM_BYTES : Cfg<BN, KBY>::SMEM_BYTES;
+  constexpr int SMEM = RS ? CfgRS<BN, P1>::SMEM_BYTES : Cfg<BN, KBY, P1>::SMEM_BYTES;
   static unsigned long long attr_mask = 0;  // the attribute is per device
   if (first_use_on_device(&attr_mask)) {
-    if (cudaFuncSetAttribute(conv_tc_kernel<BN, CL, KBY, F16, RS>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM) != cudaSuccess)
+    if (cudaFuncSetAttribute(conv_tc_kernel<BN, CL, KBY, F16, RS, P1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM) != cudaSuccess)
       return -1;
   }
   constexpr int BMT = Geo<BN>::BMT;
@@ -560,7 +581,19 @@ int launch_bn(const CUtensorMap& mXh, const CUtensorMap& mXl, const CUtensorMap&
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = CL, at[0].val.clusterDim.y = 1, at[0].val.clusterDim.z = 1;
   cfg.attrs = at, cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, CL, KBY, F16, RS>, mXh, mXl, mWh, mWl, p) == cudaSuccess ? 0 : -2;
+  return cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, CL, KBY, F16, RS, P1>, mXh, mXl, mWh, mWl, p) == cudaSuccess ? 0 : -2;
+}
+
+// the instantiation for (row-shared taps, operand format, K bytes per stage) of a channel tile / cluster / pass count
+template <int BN, int CL, bool P1>
+int launch_variant(bool rs, bool f16, int KBY, const CUtensorMap& mXh, const CUtensorMap& mXl, const CUtensorMap& mWh,
+                   const CUtensorMap& mWl, const ConvTcParams& q, int num_sms, cudaStream_t s) {
+  if (rs) return f16 ? launch_bn<BN, CL, 128, true, true, P1>(mXh, mXl, mWh, mWl, q, num_sms, s)
+                     : launch_bn<BN, CL, 128, false, true, P1>(mXh, mXl, mWh, mWl, q, num_sms, s);
+  if (f16) return KBY == 128 ? launch_bn<BN, CL, 128, true, false, P1>(mXh, mXl, mWh, mWl, q, num_sms, s)
+                             : launch_bn<BN, CL, 64, true, false, P1>(mXh, mXl, mWh, mWl, q, num_sms, s);
+  return KBY == 128 ? launch_bn<BN, CL, 128, false, false, P1>(mXh, mXl, mWh, mWl, q, num_sms, s)
+                    : launch_bn<BN, CL, 64, false, false, P1>(mXh, mXl, mWh, mWl, q, num_sms, s);
 }
 
 }  // namespace
@@ -591,6 +624,7 @@ int launch_conv_tc(const ConvTcParams& p, const void* x_hi, const void* x_lo, co
   // a 128-byte row holds 32 tf32 / 64 fp16 channels; 32-channel fp16 layers use the 64-byte (SWIZZLE_64B) rows
   const int KBY = (p.kbytes == 64 || (f16 && p.Cin % 64)) ? 64 : 128;
   if (p.kc < 1) return fail("kc must be >= 1");
+  if (p.passes != 1 && p.passes != 3) return fail("passes must be 1 or 3");
   if (p.CoutPad % conv_tc_pick_bn(p.Cout)) return fail("CoutPad must be a multiple of the channel tile");
   if (p.fin_out && (p.Cout != 128 || p.stride != 1 || p.oscale != 1 || p.stats)) return fail("fused 1x1 tail needs a plain 128-channel layer");
   const int BN = p.force_bn ? p.force_bn : (p.fin_out ? 128 : pick_bn_for_launch(p, num_sms));
@@ -653,13 +687,10 @@ int launch_conv_tc(const ConvTcParams& p, const void* x_hi, const void* x_lo, co
       encode_tmap_2d(&mWl, w_lo, (uint64_t)p.taps * p.CoutPad, p.Cin, BN / CL, KBY / eb, eb, KBY))
     return fail("cuTensorMapEncodeTiled failed");
   int rc;
-#define DVC_LAUNCH(BNv, CLv)                                                                        \
-  rc = rs ? (f16 ? launch_bn<BNv, CLv, 128, true, true>(mXh, mXl, mWh, mWl, q, num_sms, s)            \
-                 : launch_bn<BNv, CLv, 128, false, true>(mXh, mXl, mWh, mWl, q, num_sms, s))          \
-          : (f16 ? ((KBY == 128) ? launch_bn<BNv, CLv, 128, true>(mXh, mXl, mWh, mWl, q, num_sms, s)  \
-                                 : launch_bn<BNv, CLv, 64, true>(mXh, mXl, mWh, mWl, q, num_sms, s))  \
-                 : ((KBY == 128) ? launch_bn<BNv, CLv, 128, false>(mXh, mXl, mWh, mWl, q, num_sms, s) \
-                                 : launch_bn<BNv, CLv, 64, false>(mXh, mXl, mWh, mWl, q, num_sms, s)))
+  const bool one = p.passes == 1;
+#define DVC_LAUNCH(BNv, CLv)                                                                             \
+  rc = one ? launch_variant<BNv, CLv, true>(rs, f16, KBY, mXh, mXl, mWh, mWl, q, num_sms, s)             \
+           : launch_variant<BNv, CLv, false>(rs, f16, KBY, mXh, mXl, mWh, mWl, q, num_sms, s)
   if (CL == 2) {
     if (BN == 256) { DVC_LAUNCH(256, 2); } else if (BN == 128) { DVC_LAUNCH(128, 2); } else { DVC_LAUNCH(64, 2); }
   } else {

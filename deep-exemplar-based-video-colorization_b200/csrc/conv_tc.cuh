@@ -43,6 +43,7 @@ struct ConvTcParams {
   int kbytes;     // bytes of K per pipeline stage: 64 (SWIZZLE_64B, twice the stages) or 128 (SWIZZLE_128B)
   int cluster;    // 2: run as 2-CTA clusters with TMA-multicast weight tiles; 1: single CTAs
   int kc;         // 128-byte k-blocks summed in the wgmma accumulators before promotion to the fp32 register totals
+  int passes;     // MMAs per product: 3 (lo.hi + hi.lo + hi.hi, fp32-class) or 1 (hi.hi only: DVC_MATH_FP16X1)
   int rowshare;   // 1 / 2: the taps of one kernel row share one activation tile in shared memory (conv_tc.cu: CfgRS); 2 also
                   // sets the descriptors' base-offset field to the row shift; 0: one activation tile per tap
   int rs_ntx, rs_base_offset;  // filled by the launcher

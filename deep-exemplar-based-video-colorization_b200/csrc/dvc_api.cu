@@ -249,7 +249,8 @@ static int get_act(dvc_ctx* c, const std::string& name, int B, int H, int W, int
   if (mode == 3) a->h16 = (char*)p + n * 4, a->l16 = (char*)p + n * 6;
   return DVC_OK;
 }
-static bool tc_mode(const dvc_ctx* c) { return c->conv_math == DVC_MATH_TF32X3; }
+// the tensor-core layer programs (hi/lo operand planes); FP16X1 runs them with one MMA per product
+static bool tc_mode(const dvc_ctx* c) { return c->conv_math == DVC_MATH_TF32X3 || c->conv_math == DVC_MATH_FP16X1; }
 
 static int get_raw(dvc_ctx* c, const std::string& name, size_t bytes, void** out, cudaStream_t s) {
   const int sig[5] = {(int)(bytes & 0x7fffffff), 0, 0, 0, 0};
@@ -600,6 +601,7 @@ static int run_conv(dvc_ctx* c, const ConvW* w, const Act& x, Act& y, const Conv
     t.y = y.d, t.y_lo = y.lo, t.yHp = p.yHp, t.yWp = p.yWp, t.yP = p.yP, t.yC = p.yC, t.yCoff = p.yCoff;
     t.add = p.add, t.add_lo = o.add ? o.add->lo : nullptr, t.aHp = p.aHp, t.aWp = p.aWp, t.aP = p.aP, t.aC = p.aC;
     t.act = o.act, t.slope = o.slope, t.stats = o.stats, t.kc = c->tc_kc, t.cluster = c->tc_cluster, t.kbytes = c->tc_kbytes;
+    t.passes = c->conv_math == DVC_MATH_FP16X1 ? 1 : 3;
     t.tail = c->tc_tail;
     t.rowshare = c->tc_rowshare;
     t.dbg = c->tc_dbg;
@@ -1166,10 +1168,12 @@ extern "C" const char* dvc_last_error(const dvc_ctx* c) { return c ? c->err.c_st
 
 extern "C" int dvc_set_math(dvc_ctx* c, int conv_math, int corr_math) {
   if (!c) return DVC_ERR_ARG;
-  if (conv_math != DVC_MATH_FP32 && conv_math != DVC_MATH_TF32X3) return fail(c, DVC_ERR_ARG, "conv math must be DVC_MATH_FP32 or DVC_MATH_TF32X3");
-  if (conv_math != c->conv_math) c->ex_valid = false, c->warp_cache_valid = false;
+  // validate both before changing anything: a refused call leaves the context (and its cached exemplar) as it was
+  if (conv_math != DVC_MATH_FP32 && conv_math != DVC_MATH_TF32X3 && conv_math != DVC_MATH_FP16X1)
+    return fail(c, DVC_ERR_ARG, "conv math must be DVC_MATH_FP32, DVC_MATH_TF32X3 or DVC_MATH_FP16X1");
   if (corr_math != DVC_MATH_FP32 && corr_math != DVC_MATH_TF32X3 && corr_math != DVC_MATH_BF16X3 && corr_math != DVC_MATH_FP16X3)
-    return fail(c, DVC_ERR_ARG, "unknown corr math");
+    return fail(c, DVC_ERR_ARG, "corr math must be DVC_MATH_FP32, DVC_MATH_TF32X3, DVC_MATH_BF16X3 or DVC_MATH_FP16X3");
+  if (conv_math != c->conv_math) c->ex_valid = false, c->warp_cache_valid = false;
   c->conv_math = conv_math, c->corr_math = corr_math;
   return DVC_OK;
 }

@@ -15,6 +15,9 @@ LIB_PATH = os.path.join(os.path.dirname(_HERE), "lib", "libdvc.so")
 
 NET_VGG, NET_WARP, NET_COLOR = 0, 1, 2
 MATH_FP32, MATH_TF32X3, MATH_BF16X3, MATH_FP16X3 = 0, 1, 2, 3
+# convolutions only, opt-in: one MMA per product on the operand planes' hi parts (11-bit operands, the precision of
+# PyTorch's cuDNN convolutions with TF32 allowed); see include/dvc.h
+MATH_FP16X1 = 4
 
 EXPORTED = [
     "dvc_create", "dvc_destroy", "dvc_last_error", "dvc_version", "dvc_set_math", "dvc_set_weight",

@@ -50,8 +50,22 @@ typedef enum dvc_net { DVC_NET_VGG = 0, DVC_NET_WARP = 1, DVC_NET_COLOR = 2 } dv
  *   DVC_MATH_BF16X3  wgmma bf16 on hi/lo split operands (correlation only; fast mode, |df| ~ 2e-6)
  *   DVC_MATH_FP16X3  wgmma fp16 on hi/lo planes of x * 2^14 (correlation only: its operands are unit
  *                    vectors, so the power-of-two scale is exact): tf32x3's 2 x 11 bits at bf16x3's speed
+ *   DVC_MATH_FP16X1  convolutions only, opt-in fast mode: ONE MMA per product, hi * hi, on the operand planes of
+ *                    DVC_MATH_TF32X3 -- an fp16 wgmma on the fp16 planes of x * 2^e_x and w * 2^e_w (exact
+ *                    power-of-two scales), a tf32 wgmma on the tf32 planes of inputs without a known bound.  Every
+ *                    conv operand is thus rounded to 11 significant bits (round-to-nearest), as PyTorch's cuDNN
+ *                    convolutions round fp32 operands to TF32 by default (torch.backends.cudnn.allow_tf32); the
+ *                    products are exact and summed as in TF32X3.  Error per output <= ~2^-10 * sum |x| |w|.
+ *                    Activations, InstanceNorm, the small first layers and the correlation keep the default
+ *                    arithmetic.  Not accepted as corr_math (DVC_ERR_ARG).
  */
-typedef enum dvc_math { DVC_MATH_FP32 = 0, DVC_MATH_TF32X3 = 1, DVC_MATH_BF16X3 = 2, DVC_MATH_FP16X3 = 3 } dvc_math;
+typedef enum dvc_math {
+  DVC_MATH_FP32 = 0,
+  DVC_MATH_TF32X3 = 1,
+  DVC_MATH_BF16X3 = 2,
+  DVC_MATH_FP16X3 = 3,
+  DVC_MATH_FP16X1 = 4
+} dvc_math;
 
 /* ---- lifetime ------------------------------------------------------------------------------- */
 
@@ -62,7 +76,9 @@ int dvc_destroy(dvc_ctx* ctx);
 const char* dvc_last_error(const dvc_ctx* ctx); /* ctx may be NULL: last create() error */
 const char* dvc_version(void);
 
-/* Select the arithmetic of the conv layers and of the correlation (see dvc_math). */
+/* Select the arithmetic of the conv layers (FP32, TF32X3, FP16X1) and of the correlation (FP32, TF32X3, BF16X3,
+ * FP16X3; see dvc_math).  Both are validated before anything changes: a refused call leaves the context as it was.
+ * A change of conv_math invalidates the cached exemplar(s): set them again. */
 int dvc_set_math(dvc_ctx* ctx, int conv_math, int corr_math);
 
 /* ---- weights: replaces nn.Module.load_state_dict (test.py:150,158-159) ----------------------- */

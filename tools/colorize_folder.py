@@ -60,6 +60,9 @@ def main():
     ap.add_argument("--sigma-color", type=float, default=4.0)    # test.py:33
     ap.add_argument("--chunk", type=int, default=32, help="frames per device call (bounds device and host memory)")
     ap.add_argument("--workers", type=int, default=min(8, os.cpu_count() or 1), help="decode / encode threads each")
+    ap.add_argument("--fast", action="store_true",
+                    help="one MMA per convolution product (dvc.MATH_FP16X1: 11-bit conv operands, the precision of the "
+                         "reference's cuDNN convolutions on a GPU) instead of the fp32-class default")
     args = ap.parse_args()
     if args.chunk < 1:
         raise SystemExit("--chunk must be >= 1")
@@ -68,6 +71,8 @@ def main():
     from dvc.synth import make_state_dict
 
     ctx = dvc.get_context(0)
+    if args.fast:
+        ctx.set_math(conv=dvc.MATH_FP16X1)
     for net, key, path in ((dvc.NET_VGG, "vgg", args.vgg), (dvc.NET_WARP, "warp", args.warp), (dvc.NET_COLOR, "color", args.color)):
         if path:
             ctx.set_weights(net, torch.load(path, map_location="cpu"))
