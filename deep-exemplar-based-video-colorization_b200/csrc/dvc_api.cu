@@ -6,6 +6,7 @@
 //   WarpNet.forward         models/NonlocalNet.py:427-502
 //   ColorVidNet.forward     models/ColorVidNet.py:96-144
 //   frame_colorization      models/FrameColor.py:41-67, per-clip loop test.py:57-96
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <cstdio>
@@ -1683,10 +1684,13 @@ extern "C" int dvc_set_exemplars(dvc_ctx* c, const float* IB_lab, int K, int H, 
   return DVC_OK;
 }
 
-// Phase A (independent of the previous frame): VGG19 -> feature_normalize -> WarpNet A side -> correlation.
-// K > 1 (B = 1): the frame's theta against each of the K cached exemplars, into K rows of yrows / simrows.
+// Phase A (independent of the previous frame): VGG19 -> feature_normalize -> WarpNet A side -> correlation against the
+// first K cached exemplar slots.  K = 1: the B frames against slot 0.  K > 1, B = 1: the frame's theta against each of
+// the K slots (one query set shared by K batches).  B = K > 1: frame b against slot b (one clip per slot).  The results
+// fill max(B, K) rows of yrows / simrows.
 static int frames_phaseA(dvc_ctx* c, const std::string& tag, const float* IA_l, int B, int H, int W, float temperature,
                          float* yrows, float* simrows, cudaStream_t s, int arena = 0, CorrWorkspace* ws = nullptr, int K = 1) {
+  if (K > 1 && B > 1 && B != K) return fail(c, DVC_ERR_ARG, "phase A: B frames against K exemplars needs B = 1 or B = K");
   DVC_TRY(stats_begin(c, s, arena));
   const int h = H / 4, w = W / 4, N = h * w;
   Act x0;
@@ -1701,8 +1705,8 @@ static int frames_phaseA(dvc_ctx* c, const std::string& tag, const float* IA_l, 
   DVC_TRY(get_raw(c, tag + ".theta", (size_t)B * N * 256 * 4, &theta, s));
   DVC_TRY(warp_side(c, tag, n, "theta", (float*)theta, h, w, s));
   CorrParams p{};
-  p.theta = (float*)theta, p.phi = c->ex_phi, p.V = c->ex_V, p.B = K > 1 ? K : B, p.Bphi = K, p.NA = N, p.NB = N, p.C = 256;
-  p.theta_shared = K > 1;
+  p.theta = (float*)theta, p.phi = c->ex_phi, p.V = c->ex_V, p.B = K > B ? K : B, p.Bphi = K, p.NA = N, p.NB = N, p.C = 256;
+  p.theta_shared = K > 1 && B == 1;
   p.temperature = temperature, p.y = yrows, p.sim = simrows, p.argmax = nullptr;
   return run_corr(c, p, s, c->ex_version, ws);
 }
@@ -1727,28 +1731,44 @@ static int check_frame_args(dvc_ctx* c, int H, int W, float temperature, int K =
     return fail(c, DVC_ERR_STATE, "colorize: " + std::to_string(c->ex_K) + " exemplars are cached: use dvc_colorize_frames_exemplars / "
                 "dvc_colorize_clip_exemplars, or dvc_set_exemplar for a single one");
   if (K != 0 && K != c->ex_K)
-    return fail(c, DVC_ERR_SHAPE, "colorize_exemplars: K = " + std::to_string(K) + " but " + std::to_string(c->ex_K) + " exemplars are cached");
+    return fail(c, DVC_ERR_SHAPE, "colorize: the call needs " + std::to_string(K) + " exemplar slots but " + std::to_string(c->ex_K) +
+                " exemplars are cached");
   if (H != c->ex_H || W != c->ex_W) return fail(c, DVC_ERR_SHAPE, "colorize: frame size differs from the exemplar's");
   if (!(temperature > 0.f)) return fail(c, DVC_ERR_ARG, "colorize: temperature must be > 0");
   return DVC_OK;
+}
+
+// B frames, each with its own L and previous Lab: against the one cached exemplar (K = 1) or frame b against slot b (K = B,
+// one clip per slot; workspaces of their own when K > 1, so alternating with the single-exemplar calls does not reallocate)
+static int colorize_frames_impl(dvc_ctx* c, const float* IA_l, const float* IA_last_lab, int B, int K, int H, int W,
+                                float temperature, float* out_ab, float* out_warp_lab, float* out_sim, cudaStream_t s) {
+  CUDA_TRY(c, cudaSetDevice(c->device));
+  const std::string tag = K > 1 ? "frs" : "fr";
+  const int h = H / 4, w = W / 4, N = h * w;
+  void *yrows, *simrows;
+  DVC_TRY(get_raw(c, tag + ".yrows", (size_t)B * N * 16, &yrows, s));
+  DVC_TRY(get_raw(c, tag + ".simrows", (size_t)B * N * 4, &simrows, s));
+  DVC_TRY(frames_phaseA(c, tag, IA_l, B, H, W, temperature, (float*)yrows, (float*)simrows, s, 0, nullptr, K));
+  if (out_warp_lab || out_sim) {
+    launch_rows_to_nchw_up4((float*)yrows, (float*)simrows, out_warp_lab, out_sim, B, h, w, s);
+    DVC_TRY(check_launch(c, "rows_to_nchw_up4"));
+  }
+  return frames_phaseC(c, tag, IA_l, (float*)yrows, (float*)simrows, IA_last_lab, B, H, W, out_ab, s, (size_t)H * W);
 }
 
 extern "C" int dvc_colorize_frames(dvc_ctx* c, const float* IA_l, const float* IA_last_lab, int B, int H, int W,
                                    float temperature, float* out_ab, float* out_warp_lab, float* out_sim, void* stream) {
   if (!c || !IA_l || !IA_last_lab || !out_ab || B < 1) return c ? fail(c, DVC_ERR_ARG, "colorize_frames: bad argument") : DVC_ERR_ARG;
   DVC_TRY(check_frame_args(c, H, W, temperature));
-  cudaStream_t s = (cudaStream_t)stream;
-  CUDA_TRY(c, cudaSetDevice(c->device));
-  const int h = H / 4, w = W / 4, N = h * w;
-  void *yrows, *simrows;
-  DVC_TRY(get_raw(c, "fr.yrows", (size_t)B * N * 16, &yrows, s));
-  DVC_TRY(get_raw(c, "fr.simrows", (size_t)B * N * 4, &simrows, s));
-  DVC_TRY(frames_phaseA(c, "fr", IA_l, B, H, W, temperature, (float*)yrows, (float*)simrows, s));
-  if (out_warp_lab || out_sim) {
-    launch_rows_to_nchw_up4((float*)yrows, (float*)simrows, out_warp_lab, out_sim, B, h, w, s);
-    DVC_TRY(check_launch(c, "rows_to_nchw_up4"));
-  }
-  return frames_phaseC(c, "fr", IA_l, (float*)yrows, (float*)simrows, IA_last_lab, B, H, W, out_ab, s, (size_t)H * W);
+  return colorize_frames_impl(c, IA_l, IA_last_lab, B, 1, H, W, temperature, out_ab, out_warp_lab, out_sim, (cudaStream_t)stream);
+}
+
+extern "C" int dvc_colorize_frames_clips(dvc_ctx* c, const float* IA_l, const float* last_lab, int S, int H, int W, float temperature,
+                                         float* out_ab, float* out_warp_lab, float* out_sim, void* stream) {
+  if (!c || !IA_l || !last_lab || !out_ab) return c ? fail(c, DVC_ERR_ARG, "colorize_frames_clips: bad argument") : DVC_ERR_ARG;
+  if (S < 1 || S > 8) return fail(c, DVC_ERR_ARG, "colorize_frames_clips: S must be in [1, 8]");
+  DVC_TRY(check_frame_args(c, H, W, temperature, S));
+  return colorize_frames_impl(c, IA_l, last_lab, S, S, H, W, temperature, out_ab, out_warp_lab, out_sim, (cudaStream_t)stream);
 }
 
 // One frame against the K cached exemplars: phase A once at B = 1, the correlation against the K slots, phase C at
@@ -1820,13 +1840,14 @@ static void fgs_lut(float sigma_color, float lut[256]) {
   for (int d = 0; d < 256; ++d) lut[d] = (float)(-exp(-(double)d / (double)sigma_color));
 }
 
-// num_iter FGS iterations (a horizontal and a vertical sweep each) over `planes` planes in place, lambda attenuated per iteration
-static void fgs_sweeps(float* planes_data, const float* Ch, const float* Cv, float* D, int planes, int H, int W, float lambda,
-                       float lambda_attenuation, int num_iter, cudaStream_t s) {
+// num_iter FGS iterations (a horizontal and a vertical sweep each) over `planes` planes in place, lambda attenuated per
+// iteration; plane p takes the coefficients of guide p / planes_per_guide
+static void fgs_sweeps(float* planes_data, const float* Ch, const float* Cv, float* D, int planes, int planes_per_guide, int H, int W,
+                       float lambda, float lambda_attenuation, int num_iter, cudaStream_t s) {
   float lam = lambda;
   for (int n = 0; n < num_iter; ++n) {
-    launch_fgs_horizontal(planes_data, Ch, D, planes, H, W, lam, s);
-    launch_fgs_vertical(planes_data, Cv, D, planes, H, W, lam, s);
+    launch_fgs_horizontal(planes_data, Ch, D, planes, planes_per_guide, H, W, lam, s);
+    launch_fgs_vertical(planes_data, Cv, D, planes, planes_per_guide, H, W, lam, s);
     lam *= lambda_attenuation;
   }
 }
@@ -1845,15 +1866,24 @@ static void rgb_from_xyz(double inv[9]) {
 // Ring slots (frame t uses slot t & 1 or t & 3) guarded by events of the frame that last used the slot; the kernels of one
 // stage run in order on one stream, so the stage's scratch buffers (fp64 resize planes, crop, FGS Ch / Cv / D, up-sampled
 // ab) exist once.  Nothing depends on F.
-struct VideoIO {
+// One frame source: dvc_colorize_video_rgb8 has one (its frames feed all K exemplars' recurrences), dvc_colorize_videos_rgb8
+// one per clip (clip s feeds batch s of the clip loop).
+struct VideoSrc {
   const unsigned char* frames = nullptr;  // [F][Hs][Ws][3], host (pinned) or device
-  int Hs = 0, Ws = 0, Hr = 0, Wr = 0, oy = 0, ox = 0, Ho = 0, Wo = 0;
+  int Hs = 0, Ws = 0, Hr = 0, Wr = 0, oy = 0, ox = 0;
+  int ry = 0, rx = 0, ny = 0, nx = 0;
+  size_t tap0 = 0;  // its [wy | wx | 1.0] in VideoIO::taps
+  size_t src0 = 0;  // its frame in each of the two source slots
+};
+struct VideoIO {
+  std::vector<VideoSrc> clips;    // S sources
+  size_t ns_sum = 0, ns_max = 0;  // bytes of one frame of all sources / of the largest
+  int Ho = 0, Wo = 0;
   bool wls = false;
   float lambda = 0.f, sigma = 0.f;
-  unsigned char* out = nullptr;  // [K][F][Ho][Wo][3], host (pinned) or device
-  float* last_out = nullptr;     // [K][3][Ho/2][Wo/2] or nullptr
-  std::vector<double> taps;      // [wy | wx | 1.0]: uploaded once per call
-  int ry = 0, rx = 0, ny = 0, nx = 0;
+  unsigned char* out = nullptr;  // [K or S][F][Ho][Wo][3], host (pinned) or device
+  float* last_out = nullptr;     // [K or S][3][Ho/2][Wo/2] or nullptr
+  std::vector<double> taps;      // every source's [wy | wx | 1.0]: uploaded once per call
   float lut[256];
   // device workspaces
   unsigned char *src = nullptr, *crop = nullptr, *guide = nullptr, *rgb = nullptr;
@@ -1874,58 +1904,68 @@ static int video_streams(dvc_ctx* c) {
   return DVC_OK;
 }
 
-// workspaces, then the taps and the LUT on `s` (before the clip loop forks from it)
+// workspaces, then the taps and the LUT on `s` (before the clip loop forks from it).  Several clips use workspaces of their
+// own, so alternating with dvc_colorize_video_rgb8 does not reallocate.
 static int video_prologue(dvc_ctx* c, VideoIO& v, int Kb, cudaStream_t s) {
-  const size_t ns = (size_t)v.Hs * v.Ws * 3, hw = (size_t)v.Ho * v.Wo;
+  const size_t S = v.clips.size(), hw = (size_t)v.Ho * v.Wo;
+  const std::string pre = S > 1 ? "vids." : "vid.";
   auto raw = [&](const char* name, size_t bytes, auto** out) {
     void* p = nullptr;
-    const int rc = get_raw(c, name, bytes, &p, s);
+    const int rc = get_raw(c, pre + name, bytes, &p, s);
     *out = (std::remove_pointer_t<decltype(out)>)p;
     return rc;
   };
-  DVC_TRY(raw("vid.src", 2 * ns, &v.src));  // 2 slots
-  DVC_TRY(raw("vid.f0", ns * 8, &v.f0));
-  DVC_TRY(raw("vid.f1", ns * 8, &v.f1));
-  DVC_TRY(raw("vid.taps", v.taps.size() * 8, &v.dtaps));
-  DVC_TRY(raw("vid.crop", hw * 3, &v.crop));
-  DVC_TRY(raw("vid.L", 4 * hw * 4, &v.L));  // 4 slots, like the half-resolution L of the clip loop
-  DVC_TRY(raw("vid.abL", (size_t)Kb * 2 * hw * 4, &v.abL));
-  DVC_TRY(raw("vid.rgb", 2 * (size_t)Kb * hw * 3, &v.rgb));  // 2 slots
+  DVC_TRY(raw("src", 2 * v.ns_sum, &v.src));  // 2 slots of one frame per clip
+  DVC_TRY(raw("f0", v.ns_max * 8, &v.f0));    // the clips' resizes run one after another on stream I
+  DVC_TRY(raw("f1", v.ns_max * 8, &v.f1));
+  DVC_TRY(raw("taps", v.taps.size() * 8, &v.dtaps));
+  DVC_TRY(raw("crop", hw * 3, &v.crop));
+  DVC_TRY(raw("L", 4 * S * hw * 4, &v.L));  // 4 slots, like the half-resolution L of the clip loop
+  DVC_TRY(raw("abL", (size_t)Kb * 2 * hw * 4, &v.abL));
+  DVC_TRY(raw("rgb", 2 * (size_t)Kb * hw * 3, &v.rgb));  // 2 slots
   if (v.wls) {
-    DVC_TRY(raw("vid.guide", 4 * hw, &v.guide));  // 4 slots
-    DVC_TRY(raw("vid.lut", 256 * 4, &v.dlut));
-    DVC_TRY(raw("vid.Ch", hw * 4, &v.Ch));
-    DVC_TRY(raw("vid.Cv", hw * 4, &v.Cv));
-    DVC_TRY(raw("vid.D", (size_t)Kb * 2 * hw * 4, &v.D));
+    DVC_TRY(raw("guide", 4 * S * hw, &v.guide));  // 4 slots
+    DVC_TRY(raw("lut", 256 * 4, &v.dlut));
+    DVC_TRY(raw("Ch", S * hw * 4, &v.Ch));
+    DVC_TRY(raw("Cv", S * hw * 4, &v.Cv));
+    DVC_TRY(raw("D", (size_t)Kb * 2 * hw * 4, &v.D));
     CUDA_TRY(c, cudaMemcpyAsync(v.dlut, v.lut, sizeof(v.lut), cudaMemcpyHostToDevice, s));
   }
   CUDA_TRY(c, cudaMemcpyAsync(v.dtaps, v.taps.data(), v.taps.size() * 8, cudaMemcpyHostToDevice, s));
   return DVC_OK;
 }
 
-// frame t: upload (stream U) -> CenterPad resize -> L, L/2 (into the clip loop's slot Lt) and the guide (stream I);
-// records evU[t & 3], which phase A waits for
+// frame t of every clip: upload (stream U) -> CenterPad resize -> L, L/2 (clip s into plane s of the clip loop's slot Lt)
+// and the guide (stream I); records evU[t & 3], which phase A waits for
 static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
-  const size_t ns = (size_t)v.Hs * v.Ws * 3, hw = (size_t)v.Ho * v.Wo;
-  unsigned char* src = v.src + (size_t)(t & 1) * ns;
+  const size_t S = v.clips.size(), hw = (size_t)v.Ho * v.Wo;
+  unsigned char* src = v.src + (size_t)(t & 1) * v.ns_sum;
   // the source slot was last read by frame t-2's resize
   if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sU, c->evU[(t - 2) & 3], 0));
-  CUDA_TRY(c, cudaMemcpyAsync(src, v.frames + (size_t)t * ns, ns, cudaMemcpyDefault, c->sU));
+  for (const VideoSrc& k : v.clips) {
+    const size_t ns = (size_t)k.Hs * k.Ws * 3;
+    CUDA_TRY(c, cudaMemcpyAsync(src + k.src0, k.frames + (size_t)t * ns, ns, cudaMemcpyDefault, c->sU));
+  }
   CUDA_TRY(c, cudaEventRecord(c->evR[t & 3], c->sU));
   // the half-resolution L slot was last read by frame t-4's ColorVidNet / make_last, the full-resolution L and guide slots
   // by frame t-4's post-processing
   CUDA_TRY(c, cudaStreamWaitEvent(c->sI, c->evR[t & 3], 0));
   if (t >= 4) CUDA_TRY(c, cudaStreamWaitEvent(c->sI, c->evC[(t - 4) & 3], 0));
   if (t >= 4) CUDA_TRY(c, cudaStreamWaitEvent(c->sI, c->evP[(t - 4) & 3], 0));
-  // dvc_resize_antialias_crop_rgb8's kernel sequence; a zero-radius "filter" (one tap of weight 1) converts uint8 -> float64
-  double *cur = v.f0, *nxt = v.f1;
-  launch_gauss_axis_u8(src, cur, v.ny ? v.dtaps : v.dtaps + v.ny + v.nx, v.ry, 1, v.Hs, v.Ws * 3, c->sI);
-  if (v.nx) {
-    launch_gauss_axis_f64(cur, nxt, v.dtaps + v.ny, v.rx, (size_t)v.Hs, v.Ws, 3, c->sI);
-    std::swap(cur, nxt);
+  for (size_t s = 0; s < S; ++s) {
+    const VideoSrc& k = v.clips[s];
+    const double* taps = v.dtaps + k.tap0;
+    const size_t plane = (size_t)(t & 3) * S + s;
+    // dvc_resize_antialias_crop_rgb8's kernel sequence; a zero-radius "filter" (one tap of weight 1) converts uint8 -> float64
+    double *cur = v.f0, *nxt = v.f1;
+    launch_gauss_axis_u8(src + k.src0, cur, k.ny ? taps : taps + k.ny + k.nx, k.ry, 1, k.Hs, k.Ws * 3, c->sI);
+    if (k.nx) {
+      launch_gauss_axis_f64(cur, nxt, taps + k.ny, k.rx, (size_t)k.Hs, k.Ws, 3, c->sI);
+      std::swap(cur, nxt);
+    }
+    launch_zoom_crop(cur, k.Hs, k.Ws, k.Hr, k.Wr, k.oy, k.ox, v.crop, v.Ho, v.Wo, c->sI);
+    launch_rgb8_to_l_half(v.crop, v.L + plane * hw, Lt + s * (hw / 4), v.wls ? v.guide + plane * hw : nullptr, v.Ho, v.Wo, c->sI);
   }
-  launch_zoom_crop(cur, v.Hs, v.Ws, v.Hr, v.Wr, v.oy, v.ox, v.crop, v.Ho, v.Wo, c->sI);
-  launch_rgb8_to_l_half(v.crop, v.L + (size_t)(t & 3) * hw, Lt, v.wls ? v.guide + (size_t)(t & 3) * hw : nullptr, v.Ho, v.Wo, c->sI);
   DVC_TRY(check_launch(c, "video ingest"));
   CUDA_TRY(c, cudaEventRecord(c->evU[t & 3], c->sI));
   return DVC_OK;
@@ -1934,19 +1974,24 @@ static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
 // frame t, once its ColorVidNet is done (evC[t & 3]): ab x2 * 1.25, FGS, Lab -> sRGB (stream P; records evP[t & 3], which
 // the reuse of the ab slot waits for) and the download (stream D; records evD[t & 3])
 static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int Kb, int F) {
-  const size_t hw = (size_t)v.Ho * v.Wo;
+  const size_t S = v.clips.size(), hw = (size_t)v.Ho * v.Wo;
+  const float* Lfull = v.L + (size_t)(t & 3) * S * hw;
   unsigned char* rgb = v.rgb + (size_t)(t & 1) * Kb * hw * 3;
   CUDA_TRY(c, cudaStreamWaitEvent(c->sP, c->evC[t & 3], 0));
   if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sP, c->evD[(t - 2) & 3], 0));  // the rgb slot has been downloaded
   launch_upsample2(abt, v.abL, Kb * 2, v.Ho / 2, v.Wo / 2, 1.25f, c->sP);  // test.py:100-102
-  if (v.wls) {  // test.py:105-112: the a and b planes of every exemplar against the frame's one guide
-    launch_fgs_weights(v.guide + (size_t)(t & 3) * hw, v.dlut, v.Ch, v.Cv, v.Ho, v.Wo, c->sP);
-    fgs_sweeps(v.abL, v.Ch, v.Cv, v.D, Kb * 2, v.Ho, v.Wo, v.lambda, 0.25f, 3, c->sP);
+  if (v.wls) {  // test.py:105-112: one clip's a and b planes (of every exemplar) against that clip's guide, all in one launch
+    launch_fgs_weights(v.guide + (size_t)(t & 3) * S * hw, v.dlut, v.Ch, v.Cv, (int)S, v.Ho, v.Wo, c->sP);
+    fgs_sweeps(v.abL, v.Ch, v.Cv, v.D, Kb * 2, Kb * 2 / (int)S, v.Ho, v.Wo, v.lambda, 0.25f, 3, c->sP);
   }
   double inv[9];
   rgb_from_xyz(inv);
-  for (int k = 0; k < Kb; ++k)  // test.py:116-119, the frame's full-resolution L for every exemplar
-    launch_lab_to_rgb8(v.L + (size_t)(t & 3) * hw, v.abL + (size_t)k * 2 * hw, rgb + (size_t)k * hw * 3, 1, v.Ho, v.Wo, inv, c->sP);
+  if (S > 1) {  // test.py:116-119: clip s's full-resolution L with its own ab
+    launch_lab_to_rgb8(Lfull, v.abL, rgb, (int)S, v.Ho, v.Wo, inv, c->sP);
+  } else {
+    for (int k = 0; k < Kb; ++k)  // the frame's full-resolution L for every exemplar
+      launch_lab_to_rgb8(Lfull, v.abL + (size_t)k * 2 * hw, rgb + (size_t)k * hw * 3, 1, v.Ho, v.Wo, inv, c->sP);
+  }
   DVC_TRY(check_launch(c, "video post-processing"));
   CUDA_TRY(c, cudaEventRecord(c->evP[t & 3], c->sP));
   CUDA_TRY(c, cudaStreamWaitEvent(c->sD, c->evP[t & 3], 0));
@@ -1964,16 +2009,21 @@ static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int
 // K = 0: dvc_colorize_clip (one exemplar); K >= 1: dvc_colorize_clip_exemplars, K recurrences sharing the luminance
 // sequence -- phase A once per frame against the K slots, phase C at batch K, and ab of exemplar k, frame t at
 // ab_out + (k F + t) 2 H W.  The multi-exemplar workspaces have tags of their own, so alternating does not reallocate.
-// v != nullptr (dvc_colorize_video_rgb8): frame t's L comes from video_ingest instead of L_in, and video_post replaces the
+// S >= 1 (K = 0): dvc_colorize_clips, S clips, clip s against slot s -- L_in [S][F][H][W], phase A at batch S with frame s
+// against slot s, phase C at batch S with clip s's own L, ab of clip s at ab_out + (s F + t) 2 H W; several clips have
+// workspaces of their own too.  S = 0: not a several-clip call (one frame source).
+// v != nullptr (dvc_colorize_video(s)_rgb8): frame t's L comes from video_ingest instead of L_in, and video_post replaces the
 // download of ab; the recurrence state after the last frame goes to v->last_out.
-static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature, const float* first_last,
-                              int K, float* ab_out, void* stream, VideoIO* v = nullptr) {
-  const char* what = v ? "colorize_video_rgb8" : (K ? "colorize_clip_exemplars" : "colorize_clip");
+static int colorize_clip_impl(dvc_ctx* c, const char* what, const float* L_in, int F, int H, int W, float temperature,
+                              const float* first_last, int K, int S, float* ab_out, void* stream, VideoIO* v = nullptr) {
   if (!c || (!v && (!L_in || !ab_out)) || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
   if (K < 0 || K > 8) return fail(c, DVC_ERR_ARG, std::string(what) + ": K must be in [1, 8]");
-  DVC_TRY(check_frame_args(c, H, W, temperature, K));
-  const int Kb = K ? K : 1;  // batch of phase C
-  const std::string tag = K ? "clipx" : "clip";
+  if (S < 0 || S > 8 || (K && S)) return fail(c, DVC_ERR_ARG, std::string(what) + ": S must be in [1, 8], without K exemplars");
+  DVC_TRY(check_frame_args(c, H, W, temperature, K ? K : S));
+  const int nsrc = S ? S : 1;    // frame sources: batch of phase A
+  const int Kb = K ? K : nsrc;   // batch of phase C
+  const bool clips = nsrc > 1;
+  const std::string tag = K ? "clipx" : (clips ? "clips" : "clip");
   cudaStream_t s = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->device));
   DVC_TRY(clip_streams(c));
@@ -1981,7 +2031,7 @@ static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W
   const size_t hw = (size_t)H * W;
   const int N = (H / 4) * (W / 4);
   void *dL, *dlast, *dab, *yrows, *simrows;
-  DVC_TRY(get_raw(c, "clip.L", 4 * hw * 4, &dL, s));   // 4 slots
+  DVC_TRY(get_raw(c, clips ? "clips.L" : "clip.L", 4 * (size_t)nsrc * hw * 4, &dL, s));   // 4 slots of nsrc planes
   DVC_TRY(get_raw(c, tag + ".last", Kb * 3 * hw * 4, &dlast, s));
   DVC_TRY(get_raw(c, tag + ".ab", 2 * Kb * 2 * hw * 4, &dab, s));  // 2 slots
   DVC_TRY(get_raw(c, tag + ".yrows", (size_t)4 * Kb * N * 16, &yrows, s));  // 4 slots: phase A may run up to 3 frames ahead
@@ -2009,7 +2059,7 @@ static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W
     }
     for (int t = 0; t < F; ++t) {
       const int slot = t & 1;
-      float* Lt = (float*)dL + (size_t)(t & 3) * hw;
+      float* Lt = (float*)dL + (size_t)(t & 3) * nsrc * hw;
       float* abt = (float*)dab + (size_t)slot * Kb * 2 * hw;
       float* yr = (float*)yrows + (size_t)(t & 3) * Kb * N * 4;
       float* sr = (float*)simrows + (size_t)(t & 3) * Kb * N;
@@ -2020,22 +2070,24 @@ static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W
       } else {
         // ---- upload stream: the L slot was last read by frame t-4's ColorVidNet / make_last ----
         if (t >= 4) CUDA_TRY(c, cudaStreamWaitEvent(c->sU, c->evC[(t - 4) & 3], 0));
-        CUDA_TRY(c, cudaMemcpyAsync(Lt, L_in + (size_t)t * hw, hw * 4, cudaMemcpyDefault, c->sU));
+        for (int k = 0; k < nsrc; ++k)
+          CUDA_TRY(c, cudaMemcpyAsync(Lt + (size_t)k * hw, L_in + ((size_t)k * F + t) * hw, hw * 4, cudaMemcpyDefault, c->sU));
         CUDA_TRY(c, cudaEventRecord(c->evU[t & 3], c->sU));
       }
       // ---- stream A (two of them, alternating, when clip_astreams = 2): the frame-independent phase; the reuse of the
       // warp-row slot waits for frame t-4's ColorVidNet ----
       CUDA_TRY(c, cudaStreamWaitEvent(sAt, c->evU[t & 3], 0));
       if (t >= 4) CUDA_TRY(c, cudaStreamWaitEvent(sAt, c->evC[(t - 4) & 3], 0));
-      DVC_TRY(frames_phaseA(c, odd ? "clipA2" : "clipA", Lt, 1, H, W, temperature, yr, sr, sAt, odd ? 2 : 0, odd ? &c->corr_ws2 : nullptr,
-                            Kb));
+      const char* tagA = clips ? (odd ? "clipsA2" : "clipsA") : (odd ? "clipA2" : "clipA");
+      DVC_TRY(frames_phaseA(c, tagA, Lt, nsrc, H, W, temperature, yr, sr, sAt, odd ? 2 : 0, odd ? &c->corr_ws2 : nullptr, Kb));
       CUDA_TRY(c, cudaEventRecord(c->evA[t & 3], sAt));
-      // ---- stream C: the recurrent phase (the K recurrences read the frame's one L plane) ----
+      // ---- stream C: the recurrent phase (the K recurrences read the frame's one L plane, clip s its own plane s) ----
       CUDA_TRY(c, cudaStreamWaitEvent(c->sC, c->evA[t & 3], 0));
       // the ab slot has been downloaded (video: post-processed)
       if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sC, (v ? c->evP : c->evD)[(t - 2) & 3], 0));
-      DVC_TRY(frames_phaseC(c, K ? "clipCx" : "clipC", Lt, yr, sr, (float*)dlast, Kb, H, W, abt, c->sC, 0));
-      launch_make_last(Lt, 0, abt, (float*)dlast, Kb, H, W, c->sC);  // test.py:96
+      const size_t l_bstride = clips ? hw : 0;
+      DVC_TRY(frames_phaseC(c, K ? "clipCx" : (clips ? "clipCs" : "clipC"), Lt, yr, sr, (float*)dlast, Kb, H, W, abt, c->sC, l_bstride));
+      launch_make_last(Lt, l_bstride, abt, (float*)dlast, Kb, H, W, c->sC);  // test.py:96
       DVC_TRY(check_launch(c, "make_last"));
       CUDA_TRY(c, cudaEventRecord(c->evC[t & 3], c->sC));
       if (v) {
@@ -2082,13 +2134,54 @@ static int colorize_clip_impl(dvc_ctx* c, const float* L_in, int F, int H, int W
 
 extern "C" int dvc_colorize_clip(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature,
                                  const float* first_last, float* ab_out, void* stream) {
-  return colorize_clip_impl(c, L_in, F, H, W, temperature, first_last, 0, ab_out, stream);
+  return colorize_clip_impl(c, "colorize_clip", L_in, F, H, W, temperature, first_last, 0, 0, ab_out, stream);
 }
 
 extern "C" int dvc_colorize_clip_exemplars(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature,
                                            const float* first_last, int K, float* ab_out, void* stream) {
   if (c && (K < 1 || K > 8)) return fail(c, DVC_ERR_ARG, "colorize_clip_exemplars: K must be in [1, 8]");
-  return colorize_clip_impl(c, L_in, F, H, W, temperature, first_last, K, ab_out, stream);
+  return colorize_clip_impl(c, "colorize_clip_exemplars", L_in, F, H, W, temperature, first_last, K, 0, ab_out, stream);
+}
+
+extern "C" int dvc_colorize_clips(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature, const float* first_last,
+                                  int S, float* ab_out, void* stream) {
+  if (c && (S < 1 || S > 8)) return fail(c, DVC_ERR_ARG, "colorize_clips: S must be in [1, 8]");
+  return colorize_clip_impl(c, "colorize_clips", L_in, F, H, W, temperature, first_last, 0, S, ab_out, stream);
+}
+
+// One frame source of the video calls: geometry g = (Hs, Ws, Hr, Wr, oy, ox) checked as dvc_colorize_video_rgb8 documents
+// it, then appended to v with its anti-aliasing taps
+static int video_add_source(dvc_ctx* c, const char* what, VideoIO& v, const unsigned char* frames, const int g[6]) {
+  const int Hs = g[0], Ws = g[1], Hr = g[2], Wr = g[3], oy = g[4], ox = g[5];
+  if (Hs < 1 || Ws < 1 || Hr < 1 || Wr < 1 || v.Ho < 2 || v.Wo < 2 || (v.Ho & 1) || (v.Wo & 1))
+    return fail(c, DVC_ERR_SHAPE, std::string(what) + ": bad geometry (sizes >= 1, an even output size)");
+  // the output window and the resized image nest in one another along each axis: a crop of it, or a zero pad around it
+  auto nested = [](int resized, int outsz, int off) { return resized >= outsz ? off >= 0 && off <= resized - outsz : off <= 0 && off >= resized - outsz; };
+  if (!nested(Hr, v.Ho, oy) || !nested(Wr, v.Wo, ox)) return fail(c, DVC_ERR_SHAPE, std::string(what) + ": crop offset outside the resized image");
+  VideoSrc k;
+  k.frames = frames, k.Hs = Hs, k.Ws = Ws, k.Hr = Hr, k.Wr = Wr, k.oy = oy, k.ox = ox;
+  std::vector<double> wy, wx;
+  resize_taps(Hs, Ws, Hr, Wr, &wy, &k.ry, &wx, &k.rx);
+  k.ny = (int)wy.size(), k.nx = (int)wx.size();
+  k.tap0 = v.taps.size();
+  v.taps.insert(v.taps.end(), wy.begin(), wy.end());
+  v.taps.insert(v.taps.end(), wx.begin(), wx.end());
+  v.taps.push_back(1.0);
+  const size_t ns = (size_t)Hs * Ws * 3;
+  k.src0 = v.ns_sum;
+  v.ns_sum += ns, v.ns_max = std::max(v.ns_max, ns);
+  v.clips.push_back(k);
+  return DVC_OK;
+}
+
+// the checks and settings the video calls share, after their sources: output size, WLS parameters, outputs
+static int video_finish(dvc_ctx* c, const char* what, VideoIO& v, int wls, float wls_lambda, float wls_sigma, unsigned char* out,
+                        float* last_lab_out) {
+  DVC_TRY(check_frame_shape(c, what, v.Ho / 2, v.Wo / 2));
+  if (wls && !(wls_lambda >= 0.f && wls_sigma > 0.f)) return fail(c, DVC_ERR_ARG, std::string(what) + ": bad WLS parameter");
+  v.wls = wls != 0, v.lambda = wls_lambda, v.sigma = wls_sigma, v.out = out, v.last_out = last_lab_out;
+  if (v.wls) fgs_lut(wls_sigma, v.lut);
+  return DVC_OK;
 }
 
 // test.py:68-120 end to end: ingest, the clip loop and the post-processing of every frame in one pipeline (see VideoIO)
@@ -2097,26 +2190,30 @@ extern "C" int dvc_colorize_video_rgb8(dvc_ctx* c, const unsigned char* frames, 
                                        float wls_sigma, unsigned char* out, float* last_lab_out, void* stream) {
   const char* what = "colorize_video_rgb8";
   if (!c || !frames || !out || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
-  if (Hs < 1 || Ws < 1 || Hr < 1 || Wr < 1 || Ho < 2 || Wo < 2 || (Ho & 1) || (Wo & 1))
-    return fail(c, DVC_ERR_SHAPE, std::string(what) + ": bad geometry (sizes >= 1, an even output size)");
-  // the output window and the resized image nest in one another along each axis: a crop of it, or a zero pad around it
-  auto nested = [](int resized, int outsz, int off) { return resized >= outsz ? off >= 0 && off <= resized - outsz : off <= 0 && off >= resized - outsz; };
-  if (!nested(Hr, Ho, oy) || !nested(Wr, Wo, ox)) return fail(c, DVC_ERR_SHAPE, std::string(what) + ": crop offset outside the resized image");
-  DVC_TRY(check_frame_shape(c, what, Ho / 2, Wo / 2));
-  if (wls && !(wls_lambda >= 0.f && wls_sigma > 0.f)) return fail(c, DVC_ERR_ARG, std::string(what) + ": bad WLS parameter");
   VideoIO v;
-  v.frames = frames, v.Hs = Hs, v.Ws = Ws, v.Hr = Hr, v.Wr = Wr, v.oy = oy, v.ox = ox, v.Ho = Ho, v.Wo = Wo;
-  v.wls = wls != 0, v.lambda = wls_lambda, v.sigma = wls_sigma, v.out = out, v.last_out = last_lab_out;
-  std::vector<double> wy, wx;
-  resize_taps(Hs, Ws, Hr, Wr, &wy, &v.ry, &wx, &v.rx);
-  v.ny = (int)wy.size(), v.nx = (int)wx.size();
-  v.taps = wy;
-  v.taps.insert(v.taps.end(), wx.begin(), wx.end());
-  v.taps.push_back(1.0);
-  if (v.wls) fgs_lut(wls_sigma, v.lut);
+  v.Ho = Ho, v.Wo = Wo;
+  const int g[6] = {Hs, Ws, Hr, Wr, oy, ox};
+  DVC_TRY(video_add_source(c, what, v, frames, g));
+  DVC_TRY(video_finish(c, what, v, wls, wls_lambda, wls_sigma, out, last_lab_out));
   // one exemplar: the single-exemplar loop (and its workspaces), as dvc_colorize_clip
   const int K = c->ex_valid && c->ex_K > 1 ? c->ex_K : 0;
-  return colorize_clip_impl(c, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, K, nullptr, stream, &v);
+  return colorize_clip_impl(c, what, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, K, 0, nullptr, stream, &v);
+}
+
+extern "C" int dvc_colorize_videos_rgb8(dvc_ctx* c, int S, const unsigned char* const* frames, int F, const int* geom, int Ho, int Wo,
+                                        float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
+                                        unsigned char* out, float* last_lab_out, void* stream) {
+  const char* what = "colorize_videos_rgb8";
+  if (!c || !frames || !geom || !out || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
+  if (S < 1 || S > 8) return fail(c, DVC_ERR_ARG, std::string(what) + ": S must be in [1, 8]");
+  VideoIO v;
+  v.Ho = Ho, v.Wo = Wo;
+  for (int s = 0; s < S; ++s) {
+    if (!frames[s]) return fail(c, DVC_ERR_ARG, std::string(what) + ": frames[" + std::to_string(s) + "] is null");
+    DVC_TRY(video_add_source(c, what, v, frames[s], geom + 6 * s));
+  }
+  DVC_TRY(video_finish(c, what, v, wls, wls_lambda, wls_sigma, out, last_lab_out));
+  return colorize_clip_impl(c, what, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, 0, S, nullptr, stream, &v);
 }
 
 // ---- pre / post-processing around the nets (SURVEY.md §8f row 1) -----------------------------------------
@@ -2214,10 +2311,10 @@ extern "C" int dvc_fgs_filter(dvc_ctx* c, const unsigned char* dev_guide, const 
   fgs_lut(sigma_color, h_lut);
   CUDA_TRY(c, cudaMemcpyAsync(lut, h_lut, sizeof(h_lut), cudaMemcpyHostToDevice, s));
   CUDA_TRY(c, cudaStreamSynchronize(s));  // h_lut lives on this stack frame
-  launch_fgs_weights(dev_guide, (const float*)lut, (float*)Ch, (float*)Cv, H, W, s);
+  launch_fgs_weights(dev_guide, (const float*)lut, (float*)Ch, (float*)Cv, 1, H, W, s);
   DVC_TRY(check_launch(c, "fgs_weights"));
   if (dev_dst != dev_src) CUDA_TRY(c, cudaMemcpyAsync(dev_dst, dev_src, (size_t)planes * hw * 4, cudaMemcpyDeviceToDevice, s));
-  fgs_sweeps(dev_dst, (const float*)Ch, (const float*)Cv, (float*)D, planes, H, W, lambda, lambda_attenuation, num_iter, s);
+  fgs_sweeps(dev_dst, (const float*)Ch, (const float*)Cv, (float*)D, planes, planes, H, W, lambda, lambda_attenuation, num_iter, s);
   return check_launch(c, "fgs");
 }
 

@@ -266,9 +266,12 @@ void launch_lab_to_rgb8(const float* l, const float* ab, unsigned char* rgb, int
                         cudaStream_t s);
 
 // Fast Global Smoother (test.py:105-112) and the CenterPad resize (util_distortion.py:217-258): prepost.cu
-void launch_fgs_weights(const unsigned char* guide, const float* lut, float* Ch, float* Cv, int H, int W, cudaStream_t s);
-void launch_fgs_horizontal(float* cur, const float* Ch, float* D, int planes, int H, int W, float lam, cudaStream_t s);
-void launch_fgs_vertical(float* cur, const float* Cv, float* D, int planes, int H, int W, float lam, cudaStream_t s);
+// G guides [G][H][W] -> Ch / Cv [G][H][W]; the sweeps smooth plane p with the coefficients of guide p / planes_per_guide
+void launch_fgs_weights(const unsigned char* guide, const float* lut, float* Ch, float* Cv, int G, int H, int W, cudaStream_t s);
+void launch_fgs_horizontal(float* cur, const float* Ch, float* D, int planes, int planes_per_guide, int H, int W, float lam,
+                           cudaStream_t s);
+void launch_fgs_vertical(float* cur, const float* Cv, float* D, int planes, int planes_per_guide, int H, int W, float lam,
+                         cudaStream_t s);
 void launch_l_to_guide8(const float* l, unsigned char* g, size_t n, cudaStream_t s);
 // video ingest: uint8 [H][W][3] (H, W even) -> centred L [H][W] (rgb8_to_lab's plane 0), its 1/2 resolution [H/2][W/2]
 // (resize_half of that plane) and, when guide != nullptr, the WLS guide [H][W] (l_to_guide8 of the L plane)

@@ -186,6 +186,32 @@ int dvc_colorize_video_rgb8(dvc_ctx* ctx, const unsigned char* frames, int F, in
                             int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda,
                             float wls_sigma, unsigned char* out, float* last_lab_out, void* stream);
 
+/* ---- several clips in one pass, one exemplar each (a dataset or an archive: many independent runs of test.py:68-120) -----
+ * Clip s is colorized against cached exemplar slot s (dvc_set_exemplars with S images; dvc_set_exemplar is S = 1) with its
+ * own recurrence last_s = cat(L_s,t, ab_s,t) (test.py:96).  VGG19, the WarpNet query side and the correlation run at batch S
+ * with frame s against slot s, ColorVidNet at batch S -- ColorVidNet is recurrent, so frames of other clips are what fills
+ * its low-resolution layers.  All clips of a call share the frame size, the temperature and F; clips of different lengths
+ * stream in chunks and leave between calls.  S = 1 gives the bits of the single-exemplar calls; with S > 1 a clip's results
+ * equal its solo run up to the InstanceNorm summation order and the device-derived fp16 scales that ColorVidNet shares
+ * across its batch.  S outside [1, 8] is DVC_ERR_ARG; an S other than the cached exemplar count or a frame size other than
+ * the exemplars' is DVC_ERR_SHAPE (so S clips with several exemplars each are refused).  A refused call launches nothing. */
+
+/* dvc_colorize_frames for S frames, frame s against slot s: dev_IA_l [S,1,H,W]; dev_last_lab [S,3,H,W]; dev_out_ab [S,2,H,W];
+ * optional dev_out_warp_lab [S,3,H,W] and dev_out_sim [S,1,H,W] (may be NULL).  All device pointers. */
+int dvc_colorize_frames_clips(dvc_ctx* ctx, const float* dev_IA_l, const float* dev_last_lab, int S, int H, int W, float temperature,
+                              float* dev_out_ab, float* dev_out_warp_lab, float* dev_out_sim, void* stream);
+/* dvc_colorize_clip for S clips: L [S,F,1,H,W]; first_last_lab NULL (zeros) or [S,3,H,W]; ab [S,F,2,H,W].  Host (pinned)
+ * or device memory.  Synchronises `stream` before returning. */
+int dvc_colorize_clips(dvc_ctx* ctx, const float* L, int F, int H, int W, float temperature, const float* first_last_lab, int S,
+                       float* ab, void* stream);
+/* dvc_colorize_video_rgb8 for S clips: frames[s] points to clip s's [F,Hs_s,Ws_s,3] uint8 frames (the source sizes may differ
+ * between clips); geom [S][6] holds (Hs, Ws, Hr, Wr, oy, ox) of each clip, each checked as dvc_colorize_video_rgb8 checks
+ * its own; out [S,F,Ho,Wo,3]; first_last_lab and last_lab_out NULL or [S,3,Ho/2,Wo/2].  A null frames[s] is DVC_ERR_ARG.
+ * Device memory does not depend on F.  Synchronises `stream` before returning. */
+int dvc_colorize_videos_rgb8(dvc_ctx* ctx, int S, const unsigned char* const* frames, int F, const int* geom, int Ho, int Wo,
+                             float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
+                             unsigned char* out, float* last_lab_out, void* stream);
+
 /* ---- pre / post-processing around the nets (SURVEY.md §8f row 1) ------------------------------ */
 
 /* F.interpolate(x, scale_factor=0.5, mode="bilinear") -- test.py:58,71.  dev_src [planes,H,W] (H, W even) ->

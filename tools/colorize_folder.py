@@ -15,6 +15,12 @@ by the chunk size, not by the clip length.  Consecutive frames of one source siz
 Several --ref images (test.py:168-181 colorizes the clip once per reference) take one pass: dvc_set_exemplars and the
 exemplar-independent half of every frame computed once; each exemplar's frames go to --out/<exemplar file name>/.
 
+Several --clip folders (at most 8) take one pass too, with exactly one --ref per clip: clip s against --ref s, its frames
+to --out/<clip folder name>/.  Every call (dvc_colorize_videos_rgb8) takes the same number of frames n from each clip that
+has frames left: n = min(--chunk, the run of frames of one source size each such clip has next).  When a clip runs out,
+it leaves: the others continue with dvc_set_exemplars of their references and their rows of the previous call's
+last_lab_out.  (Several clips with several references each are refused.)
+
 What the reference does and this script does not: the AVI writer (folder2vid).  Image decode / encode stays on the host
 (PIL), as in the reference.  Without checkpoints (none ship with the reference tree) pass --seeded-weights to run the
 pipeline on the seeded random weights of dvc/synth.py (useful as a smoke run only).
@@ -44,12 +50,46 @@ def save_png(img, path):
     Image.fromarray(img).save(path)
 
 
+class Source:
+    """One clip folder: its frame names in order and a queue of decodes running ahead of the device."""
+
+    def __init__(self, folder, decode, chunk):
+        self.folder, self.decode, self.chunk = folder, decode, chunk
+        names = sorted(os.listdir(folder), key=lambda f: int("".join(filter(str.isdigit, f)) or -1))
+        self.todo = iter(names)
+        self.pending = collections.deque()  # (name, decode future), at most two chunks ahead of the device
+
+    def read_ahead(self):
+        for n in self.todo:
+            self.pending.append((n, self.decode.submit(load_rgb8, os.path.join(self.folder, n))))
+            if len(self.pending) >= 2 * self.chunk:
+                break
+
+    def run(self):
+        """Number of decoded frames of one source size at the front, up to the chunk size (0: the clip is done)."""
+        self.read_ahead()
+        n = 0
+        while n < min(self.chunk, len(self.pending)):
+            if n and self.pending[n][1].result().shape != self.pending[0][1].result().shape:
+                break
+            n += 1
+        return n
+
+    def take(self, n):
+        chunk = [(name, f.result()) for name, f in (self.pending.popleft() for _ in range(n))]
+        self.read_ahead()
+        return chunk
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--clip", required=True, help="folder of frames (sorted by the digits in the file names, test.py:41)")
+    ap.add_argument("--clip", required=True, nargs="+",
+                    help="folder(s) of frames (sorted by the digits in the file names, test.py:41); with several (at most 8), "
+                         "one pass colorizes them all, each against its own --ref, into --out/<clip folder name>/")
     ap.add_argument("--ref", required=True, nargs="+",
                     help="exemplar image(s); with several (at most 8), one pass colorizes the clip against each and writes "
-                         "--out/<exemplar name>/ (test.py:168-181 loops over a folder of references)")
+                         "--out/<exemplar name>/ (test.py:168-181 loops over a folder of references); with several --clip "
+                         "folders, exactly one per clip")
     ap.add_argument("--out", required=True)
     ap.add_argument("--vgg"), ap.add_argument("--warp"), ap.add_argument("--color")
     ap.add_argument("--seeded-weights", action="store_true")
@@ -58,7 +98,7 @@ def main():
     ap.add_argument("--no-wls", action="store_true", help="skip the Fast Global Smoother (test.py:31 wls_filter_on)")
     ap.add_argument("--lambda-value", type=float, default=500.0)  # test.py:32
     ap.add_argument("--sigma-color", type=float, default=4.0)    # test.py:33
-    ap.add_argument("--chunk", type=int, default=32, help="frames per device call (bounds device and host memory)")
+    ap.add_argument("--chunk", type=int, default=32, help="frames per clip and device call (bounds device and host memory)")
     ap.add_argument("--workers", type=int, default=min(8, os.cpu_count() or 1), help="decode / encode threads each")
     ap.add_argument("--fast", action="store_true",
                     help="one MMA per convolution product (dvc.MATH_FP16X1: 11-bit conv operands, the precision of the "
@@ -66,6 +106,12 @@ def main():
     args = ap.parse_args()
     if args.chunk < 1:
         raise SystemExit("--chunk must be >= 1")
+    S = len(args.clip)
+    if S > 8:
+        raise SystemExit("--clip: at most 8 folders in one pass")
+    if S > 1 and len(args.ref) != S:
+        raise SystemExit("--ref: with several --clip folders, give exactly one exemplar per clip (several clips with several "
+                         "references each are not supported)")
 
     import dvc
     from dvc.synth import make_state_dict
@@ -81,77 +127,79 @@ def main():
         else:
             raise SystemExit(f"--{key} checkpoint missing (or pass --seeded-weights)")
 
-    names = sorted(os.listdir(args.clip), key=lambda f: int("".join(filter(str.isdigit, f)) or -1))
     H, W = args.image_size
     if H % 16 or W % 32:
         raise SystemExit("--image-size must have H % 16 == 0 and W % 32 == 0 (the networks run at half of it)")
     # test.py:44-46 + 57-66: CenterPad(image_size) + CenterCrop(image_size) of the exemplar(s), Lab, 1/2, features once
     refs = torch.stack([ctx.centerpad_rgb8(torch.from_numpy(load_rgb8(r).copy()).cuda(), (H, W)) for r in args.ref])  # [K,H,W,3]
-    if len(args.ref) == 1:
-        ctx.set_exemplar(ctx.resize_half(ctx.rgb8_to_lab(refs)))
+    ref_lab = ctx.resize_half(ctx.rgb8_to_lab(refs))
+    if S > 1:  # clip s against exemplar s, every clip's recurrence in one pass
+        ctx.set_exemplars(ref_lab)
+        outs = [os.path.join(args.out, os.path.basename(os.path.normpath(d))) for d in args.clip]
+        if len(set(outs)) != len(outs):
+            raise SystemExit("--clip: the folder names must differ (they name the output folders)")
+    elif len(args.ref) == 1:
+        ctx.set_exemplar(ref_lab)
         outs = [args.out]
     else:  # every exemplar's recurrence in one pass over the clip
-        ctx.set_exemplars(ctx.resize_half(ctx.rgb8_to_lab(refs)))
+        ctx.set_exemplars(ref_lab)
         outs = [os.path.join(args.out, os.path.splitext(os.path.basename(r))[0]) for r in args.ref]
         if len(set(outs)) != len(outs):
             raise SystemExit("--ref: the exemplar file names must differ (they name the output folders)")
     for d in outs:
         os.makedirs(d, exist_ok=True)
     wls = None if args.no_wls else (args.lambda_value, args.sigma_color)
-    K, C = len(outs), args.chunk
+    C = args.chunk
 
     decode, encode = ThreadPoolExecutor(args.workers), ThreadPoolExecutor(args.workers)
-    pending = collections.deque()  # (name, decode future), at most two chunks ahead of the device
-    todo = iter(names)
-
-    def read_ahead():
-        for n in todo:
-            pending.append((n, decode.submit(load_rgb8, os.path.join(args.clip, n))))
-            if len(pending) >= 2 * C:
-                break
-
-    def next_chunk():
-        """Up to C consecutive decoded frames of one source size: [(name, array)]."""
-        read_ahead()
-        chunk = []
-        while pending and len(chunk) < C:
-            img = pending[0][1].result()
-            if chunk and img.shape != chunk[0][1].shape:
-                break
-            chunk.append((pending.popleft()[0], img))
-            read_ahead()
-        return chunk
-
-    ring_in = [None, None]   # pinned [C,Hs,Ws,3] frame chunks
-    ring_out = [None, None]  # pinned [K,C,H,W,3] result chunks and the encodes still reading them
+    sources = [Source(d, decode, C) for d in args.clip]
+    active = list(range(S))  # clips with frames left; row j of a call's output and last_lab_out is clip active[j]
+    ring_in = [[None] * S, [None] * S]  # pinned [C,Hs,Ws,3] frame chunks per clip
+    ring_out = [None, None]  # pinned [rows,n,H,W,3] result chunks and the encodes still reading them
     writes = [[], []]
-    last, done, i = None, 0, 0
+    last, done, i = None, [0] * S, 0
     while True:
-        chunk = next_chunk()
-        if not chunk:
+        runs = [sources[s].run() for s in active]
+        keep = [j for j, r in enumerate(runs) if r > 0]
+        if not keep:
             break
-        n, shape, slot = len(chunk), chunk[0][1].shape, i & 1
-        if ring_in[slot] is None or tuple(ring_in[slot].shape[1:]) != shape:
-            ring_in[slot] = torch.empty((C,) + shape, dtype=torch.uint8).pin_memory()
-        for t, (_, img) in enumerate(chunk):
-            ring_in[slot][t].copy_(torch.from_numpy(img))
+        if len(keep) < len(active):  # a clip ran out of frames: the others continue with their exemplars and states
+            active, runs = [active[j] for j in keep], [runs[j] for j in keep]
+            last = last[keep] if last is not None else None
+            ctx.set_exemplars(ref_lab[active])
+        n, slot = min(runs), i & 1
+        chunks = [sources[s].take(n) for s in active]
+        for s, chunk in zip(active, chunks):
+            shape = chunk[0][1].shape
+            if ring_in[slot][s] is None or tuple(ring_in[slot][s].shape[1:]) != shape:
+                ring_in[slot][s] = torch.empty((C,) + shape, dtype=torch.uint8).pin_memory()
+            for t, (_, img) in enumerate(chunk):
+                ring_in[slot][s][t].copy_(torch.from_numpy(img))
         for f in writes[slot]:  # the encodes of chunk i-2 still read this output slot
             f.result()
-        if ring_out[slot] is None or ring_out[slot].shape[1] != n:
-            ring_out[slot] = torch.empty(K, n, H, W, 3, dtype=torch.uint8).pin_memory()
-        out, last = ctx.colorize_video_rgb8(ring_in[slot][:n], (H, W), args.temperature, first_last_lab=last, wls=wls,
-                                            out=ring_out[slot], return_last=True)
+        rows = len(outs) if S == 1 else len(active)
+        if ring_out[slot] is None or tuple(ring_out[slot].shape[:2]) != (rows, n):
+            ring_out[slot] = torch.empty(rows, n, H, W, 3, dtype=torch.uint8).pin_memory()
+        if S == 1:
+            out, last = ctx.colorize_video_rgb8(ring_in[slot][0][:n], (H, W), args.temperature, first_last_lab=last, wls=wls,
+                                                out=ring_out[slot], return_last=True)
+            dests = [(outs[k], chunks[0]) for k in range(rows)]
+        else:
+            out, last = ctx.colorize_videos_rgb8([ring_in[slot][s][:n] for s in active], (H, W), args.temperature,
+                                                 first_last_lab=last, wls=wls, out=ring_out[slot], return_last=True)
+            dests = [(outs[s], chunk) for s, chunk in zip(active, chunks)]
         arr = out.numpy()
-        writes[slot] = [encode.submit(save_png, arr[k, t], os.path.join(outs[k], os.path.splitext(name)[0] + ".png"))
-                        for k in range(K) for t, (name, _) in enumerate(chunk)]
-        done += n
+        writes[slot] = [encode.submit(save_png, arr[r, t], os.path.join(d, os.path.splitext(name)[0] + ".png"))
+                        for r, (d, chunk) in enumerate(dests) for t, (name, _) in enumerate(chunk)]
+        for s in active:
+            done[s] += n
         i += 1
     for ws in writes:
         for f in ws:
             f.result()
     decode.shutdown(), encode.shutdown()
-    for d in outs:
-        print(f"{done} frames -> {d}")
+    for r, d in enumerate(outs):
+        print(f"{done[0 if S == 1 else r]} frames -> {d}")
 
 
 if __name__ == "__main__":
