@@ -32,7 +32,7 @@ __global__ void __launch_bounds__(256) corr_simt_kernel(const CorrParams p) {
   const int b = blockIdx.y;
   const int bphi = (p.Bphi == 1) ? 0 : b;
   const int m0 = blockIdx.x * BM;
-  const float* __restrict__ th = p.theta + (size_t)(p.theta_shared ? 0 : b) * p.NA * p.C;
+  const float* __restrict__ th = p.theta + (size_t)p.qsrc.at(b) * p.NA * p.C;
   const float* __restrict__ ph = p.phi + (size_t)bphi * p.NB * p.C;
   const float4* __restrict__ Vg = reinterpret_cast<const float4*>(p.V) + (size_t)bphi * p.NB;
 

@@ -97,7 +97,7 @@ struct SplitOut {
 
 struct TcParams {
   int NA, NB, B, Bphi, C;
-  int a_bstride;  // query rows between batches in the A planes: NA, or 0 when every batch shares one query set
+  PlaneSrc qsrc;  // batch b reads query set qsrc.at(b): rows qsrc.at(b) * NA .. + NA of the A planes
   int tiles_per_split;
   float sc;  // log2(e) / T
   const float* row_sc;  // optional per-query-row log2(e) / T_i (overrides sc): the contextual loss normalises every row by its own minimum distance
@@ -241,6 +241,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
       // ================= TMA producer (warp-convergent loop, one elected lane issues) =================
       int stage = 0;
       uint32_t phase = 0;
+      const int arow0 = p.qsrc.at(b) * p.NA;
       for (int t = 0; t < ntiles; ++t) {
         const int col0 = bphi * p.NB + (t0 + t) * BN;
         for (int kb = 0; kb < nkb; ++kb) {
@@ -248,8 +249,8 @@ __global__ void __launch_bounds__(NTHREADS, 1)
           if (tc::elect_one()) {
             uint8_t* st = smem + stage * STAGE_BYTES;
             tc::mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
-            tc::tma_load_2d(st, &tmAh, &full[stage], kb * KB, b * p.a_bstride + m0);
-            tc::tma_load_2d(st + A_BYTES, &tmAl, &full[stage], kb * KB, b * p.a_bstride + m0);
+            tc::tma_load_2d(st, &tmAh, &full[stage], kb * KB, arow0 + m0);
+            tc::tma_load_2d(st + A_BYTES, &tmAl, &full[stage], kb * KB, arow0 + m0);
             if (CL == 1) {
               tc::tma_load_2d(st + 2 * A_BYTES, &tmBh, &full[stage], kb * KB, col0);
               tc::tma_load_2d(st + 2 * A_BYTES + B_BYTES, &tmBl, &full[stage], kb * KB, col0);
@@ -421,9 +422,9 @@ struct ScreenCfg {
 
 struct ScreenParams {
   int NA, NB, B, Bphi, C;
-  int a_bstride;  // query rows between batches in the A plane and the query norms: NA, or 0 for one shared query set
+  PlaneSrc qsrc;  // batch b reads query set qsrc.at(b) of the A plane and the query norms
   int tiles_per_split;
-  const float* nd_a;   // [B*NA] (one shared query set: [NA])   ||dropped part|| of every query row
+  const float* nd_a;   // [query sets * NA]   ||dropped part|| of every query row
   const float* nh_a;   //                                       ||hi part||
   const unsigned int* nd_b_max;  // float bits: max over reference rows of ||dropped part||
   const unsigned int* nh_b_max;  //             max over reference rows of ||hi part||
@@ -480,7 +481,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
       uint32_t phase = 0;
       if (ntiles > 0 && tc::elect_one()) {  // the query tile: loaded once, resident for the whole sweep
         tc::mbar_arrive_expect_tx(afull, A_RES);
-        for (int kb = 0; kb < nkb; ++kb) tc::tma_load_2d(smem + kb * A_BYTES, &tmAh, afull, kb * KB, b * p.a_bstride + m0);
+        for (int kb = 0; kb < nkb; ++kb) tc::tma_load_2d(smem + kb * A_BYTES, &tmAh, afull, kb * KB, p.qsrc.at(b) * p.NA + m0);
       }
       __syncwarp();
       for (int t = 0; t < ntiles; ++t) {
@@ -518,7 +519,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
     int cnt[2] = {0, 0};  // entries appended (only the first SCREEN_K are stored: cnt > SCREEN_K = overflow)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {  // candidate threshold in accumulator units (scores there are true scores * 2^28)
-      const size_t grow = (size_t)b * p.a_bstride + min(m0 + rl + 8 * h, p.NA - 1);
+      const size_t grow = (size_t)p.qsrc.at(b) * p.NA + min(m0 + rl + 8 * h, p.NA - 1);
       thr[h] = screen_threshold(__ldg(p.nd_a + grow), __ldg(p.nh_a + grow), __uint_as_float(__ldg(p.nd_b_max)),
                                 __uint_as_float(__ldg(p.nh_b_max))) * 268435456.0f;
     }
@@ -614,7 +615,7 @@ __global__ void __launch_bounds__(256) corr_rescore_kernel(const float* __restri
   const int bphi = (p.Bphi == 1) ? 0 : b;
   const float* ph = phi + (size_t)bphi * p.NB * 256;
   const float4* Vg = V + (size_t)bphi * p.NB;
-  const int ra = b * p.a_bstride + (r - b * p.NA);  // query row in theta and in the query norms
+  const int ra = p.qsrc.at(b) * p.NA + (r - b * p.NA);  // query row in theta and in the query norms
   const float4 a0 = __ldg(reinterpret_cast<const float4*>(theta + (size_t)ra * 256) + lane);
   const float4 a1 = __ldg(reinterpret_cast<const float4*>(theta + (size_t)ra * 256) + 32 + lane);
   auto score = [&](int col) {
@@ -830,9 +831,8 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
   const int fmt = math == 1 ? 0 : (math == 2 ? 1 : 2);  // DVC_MATH_TF32X3 / BF16X3 / FP16X3
   if (p.C < 64 || p.C % 64 || p.C > 4096) return fail("C must be a multiple of 64 (<= 4096)");
   const int eb = tf32 ? 4 : 2;
-  if (p.theta_shared && p.Bphi != p.B) return fail("a shared query set needs Bphi == B");
-  // query rows in theta / the A planes: one set for all batches when it is shared (prepared once, not B times)
-  const int qrows = (p.theta_shared ? 1 : p.B) * p.NA, a_bstride = p.theta_shared ? 0 : p.NA;
+  // query rows in theta / the A planes: each query set once, however many batches read it
+  const int qrows = p.qsrc.count(p.B) * p.NA;
   const size_t ea = (size_t)qrows * p.C, ephi = (size_t)p.Bphi * p.NB * p.C;
   void *Ah, *Al, *Bh, *Bl, *part;
   if (ws_get(ws, 0, ea * eb, &Ah) || ws_get(ws, 1, ea * eb, &Al) || ws_get(ws, 2, ephi * eb, &Bh) || ws_get(ws, 3, ephi * eb, &Bl))
@@ -887,7 +887,7 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
     if (encode_tmap_2d(&mA, Ah, (uint64_t)qrows, p.C, BM, 64, 2) || encode_tmap_2d(&mB, Bh, (uint64_t)rphi, p.C, BN / cl, 64, 2))
       return fail("cuTensorMapEncodeTiled failed");
     ScreenParams sp;
-    sp.NA = p.NA, sp.NB = p.NB, sp.B = p.B, sp.Bphi = p.Bphi, sp.C = p.C, sp.a_bstride = a_bstride, sp.tiles_per_split = tps;
+    sp.NA = p.NA, sp.NB = p.NB, sp.B = p.B, sp.Bphi = p.Bphi, sp.C = p.C, sp.qsrc = p.qsrc, sp.tiles_per_split = tps;
     sp.nd_a = nd_a, sp.nh_a = nh_a, sp.nd_b_max = cells + 2, sp.nh_b_max = cells + 3;
     sp.pm = (float*)cand;
     sp.pcnt = (int*)(sp.pm + (size_t)sparts * rows);
@@ -928,7 +928,7 @@ int launch_corr_tc(const CorrParams& p, int math, int cluster, int screen, CorrW
     return fail("cuTensorMapEncodeTiled failed");
 
   TcParams tp;
-  tp.NA = p.NA, tp.NB = p.NB, tp.B = p.B, tp.Bphi = p.Bphi, tp.C = p.C, tp.a_bstride = a_bstride, tp.tiles_per_split = tps;
+  tp.NA = p.NA, tp.NB = p.NB, tp.B = p.B, tp.Bphi = p.Bphi, tp.C = p.C, tp.qsrc = p.qsrc, tp.tiles_per_split = tps;
   tp.sc = 1.4426950408889634f / p.temperature;
   tp.row_sc = p.row_scale;
   tp.out_scale = fmt == 2 ? 3.725290298461914e-09f /* 2^-28 */ : 1.0f;

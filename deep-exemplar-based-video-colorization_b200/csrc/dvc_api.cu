@@ -1492,19 +1492,20 @@ extern "C" int dvc_debug_conv2d(dvc_ctx* c, int net, const char* name, const flo
 }
 
 // ---- stand-alone correlation ---------------------------------------------------------------------
-// theta_shared: one query set [1][C][NA] against B = Bphi reference sets (dvc_corr_softmax_warp_exemplars)
+// one_query_set: one query set [1][C][NA] against B = Bphi reference sets (dvc_corr_softmax_warp_exemplars)
 static int corr_standalone(dvc_ctx* c, const float* theta_hat, const float* phi_hat, const float* V, int B, int Bphi,
-                           bool theta_shared, int NA, int NB, int C, float temperature, float* y, float* sim, int32_t* argmax,
+                           bool one_query_set, int NA, int NB, int C, float temperature, float* y, float* sim, int32_t* argmax,
                            void* stream) {
   if (!c || !theta_hat || !phi_hat || !V || !y || !sim) return c ? fail(c, DVC_ERR_ARG, "corr: bad argument") : DVC_ERR_ARG;
   if (C < 64 || C % 64 || C > 4096) return fail(c, DVC_ERR_SHAPE, "corr: C must be a multiple of 64 (WarpNet.inter_channels is 256)");
   if (C != 256 && c->corr_math == DVC_MATH_FP32) return fail(c, DVC_ERR_SHAPE, "corr: the CUDA-core twin is built for C = 256");
   if (B < 1 || NA < 1 || NB < 1 || (Bphi != B && Bphi != 1)) return fail(c, DVC_ERR_SHAPE, "corr: bad sizes");
   if (!(temperature > 0.f)) return fail(c, DVC_ERR_ARG, "corr: temperature must be > 0");
-  if (theta_shared && c->corr_peers.n > 0) return fail(c, DVC_ERR_STATE, "corr: peer outputs are not supported with several exemplars");
+  if (one_query_set && c->corr_peers.n > 0) return fail(c, DVC_ERR_STATE, "corr: peer outputs are not supported with several exemplars");
   cudaStream_t s = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->device));
-  const int Bq = theta_shared ? 1 : B;  // query sets
+  const PlaneSrc qsrc = one_query_set ? PlaneSrc::shared() : PlaneSrc::identity();
+  const int Bq = qsrc.count(B);  // query sets
   void *th, *ph, *V4, *y4;
   DVC_TRY(get_raw(c, "corr.theta", (size_t)Bq * NA * C * 4, &th, s));
   DVC_TRY(get_raw(c, "corr.phi", (size_t)Bphi * NB * C * 4, &ph, s));
@@ -1523,7 +1524,7 @@ static int corr_standalone(dvc_ctx* c, const float* theta_hat, const float* phi_
   }
   CorrParams p{};
   p.theta = (float*)th, p.phi = (float*)ph, p.V = (float*)V4, p.B = B, p.Bphi = Bphi, p.NA = NA, p.NB = NB, p.C = C;
-  p.theta_shared = theta_shared;
+  p.qsrc = qsrc;
   p.temperature = temperature, p.y = (float*)y4, p.sim = sim, p.argmax = argmax;
   if (c->corr_peers.n > 0) {
     if (B != 1) return fail(c, DVC_ERR_SHAPE, "corr: peer outputs need B = 1");
@@ -1684,13 +1685,46 @@ extern "C" int dvc_set_exemplars(dvc_ctx* c, const float* IB_lab, int K, int H, 
   return DVC_OK;
 }
 
-// Phase A (independent of the previous frame): VGG19 -> feature_normalize -> WarpNet A side -> correlation against the
-// first K cached exemplar slots.  K = 1: the B frames against slot 0.  K > 1, B = 1: the frame's theta against each of
-// the K slots (one query set shared by K batches).  B = K > 1: frame b against slot b (one clip per slot).  The results
-// fill max(B, K) rows of yrows / simrows.
-static int frames_phaseA(dvc_ctx* c, const std::string& tag, const float* IA_l, int B, int H, int W, float temperature,
-                         float* yrows, float* simrows, cudaStream_t s, int arena = 0, CorrWorkspace* ws = nullptr, int K = 1) {
-  if (K > 1 && B > 1 && B != K) return fail(c, DVC_ERR_ARG, "phase A: B frames against K exemplars needs B = 1 or B = K");
+// Rows of a call over S frame sources (clips), clip s with K[s] exemplar rows (K == nullptr: one row per source).  Row r is
+// one (clip, exemplar) pair: the rows of clip s are contiguous and in its exemplar order, row r reads cached exemplar slot r
+// (slot 0 for every row while a single exemplar is cached) and src->at(r) is its clip.  Returns R = sum K[s].
+static int row_table(int S, const int* K, PlaneSrc* src) {
+  if (!K) {
+    *src = PlaneSrc::identity();
+    return S;
+  }
+  *src = PlaneSrc::shared();
+  int R = 0;
+  for (int s = 0; s < S; ++s)
+    for (int k = 0; k < K[s]; ++k, ++R)
+      if (R < 8) src->set(R, s);
+  return R;
+}
+
+// the per-clip exemplar counts of the *_clips_exemplars entry points: S clips in [1, 8], every K[s] >= 1, sum K[s] <= 8
+static int check_counts(dvc_ctx* c, const char* what, int S, const int* K) {
+  if (S < 1 || S > 8) return fail(c, DVC_ERR_ARG, std::string(what) + ": S must be in [1, 8]");
+  if (!K) return fail(c, DVC_ERR_ARG, std::string(what) + ": K is null");
+  int R = 0;
+  for (int s = 0; s < S; ++s) {
+    if (K[s] < 1 || K[s] > 8) return fail(c, DVC_ERR_ARG, std::string(what) + ": K[" + std::to_string(s) + "] must be in [1, 8]");
+    R += K[s];
+  }
+  if (R > 8) return fail(c, DVC_ERR_ARG, std::string(what) + ": at most 8 rows (sum of K) per call, got " + std::to_string(R));
+  return DVC_OK;
+}
+// K, or nullptr when every clip has one exemplar row: the several-clip call itself (its workspaces and its bits)
+static const int* counts_or_null(int S, const int* K) {
+  for (int s = 0; s < S; ++s)
+    if (K[s] != 1) return K;
+  return nullptr;
+}
+
+// Phase A (independent of the previous frame): VGG19 -> feature_normalize -> WarpNet A side at batch B, one frame per
+// source, then the correlation of R rows: row r is frame src.at(r) against cached exemplar slot r, or against slot 0 for
+// every row while one exemplar is cached.  The results fill R rows of yrows / simrows.
+static int frames_phaseA(dvc_ctx* c, const std::string& tag, const float* IA_l, int B, int R, const PlaneSrc& src, int H, int W,
+                         float temperature, float* yrows, float* simrows, cudaStream_t s, int arena = 0, CorrWorkspace* ws = nullptr) {
   DVC_TRY(stats_begin(c, s, arena));
   const int h = H / 4, w = W / 4, N = h * w;
   Act x0;
@@ -1705,20 +1739,20 @@ static int frames_phaseA(dvc_ctx* c, const std::string& tag, const float* IA_l, 
   DVC_TRY(get_raw(c, tag + ".theta", (size_t)B * N * 256 * 4, &theta, s));
   DVC_TRY(warp_side(c, tag, n, "theta", (float*)theta, h, w, s));
   CorrParams p{};
-  p.theta = (float*)theta, p.phi = c->ex_phi, p.V = c->ex_V, p.B = K > B ? K : B, p.Bphi = K, p.NA = N, p.NB = N, p.C = 256;
-  p.theta_shared = K > 1 && B == 1;
+  p.theta = (float*)theta, p.phi = c->ex_phi, p.V = c->ex_V, p.B = R, p.Bphi = c->ex_K, p.NA = N, p.NB = N, p.C = 256;
+  p.qsrc = src;
   p.temperature = temperature, p.y = yrows, p.sim = simrows, p.argmax = nullptr;
   return run_corr(c, p, s, c->ex_version, ws);
 }
 
-// Phase C (the recurrent part): ColorVidNet on [L, warped ab, similarity, previous Lab] (FrameColor.py:63-65).
-// l_bstride: floats between the L planes of consecutive batches (0: one frame's L for all K exemplars' recurrences)
+// Phase C (the recurrent part): ColorVidNet on [L, warped ab, similarity, previous Lab] (FrameColor.py:63-65) of B rows,
+// row b reading luminance plane lsrc.at(b) of IA_l
 static int frames_phaseC(dvc_ctx* c, const std::string& tag, const float* IA_l, const float* yrows, const float* simrows,
-                         const float* IA_last_lab, int B, int H, int W, float* out_ab, cudaStream_t s, size_t l_bstride) {
+                         const float* IA_last_lab, int B, int H, int W, float* out_ab, cudaStream_t s, const PlaneSrc& lsrc) {
   DVC_TRY(stats_begin(c, s, 1));
   Act in0;
   DVC_TRY(get_act(c, tag + ".in0", B, H, W, 8, 1, &in0, s));
-  launch_build_color_input(IA_l, l_bstride, yrows, simrows, IA_last_lab, in0.d, B, H, W, 1, s);
+  launch_build_color_input(IA_l, lsrc, yrows, simrows, IA_last_lab, in0.d, B, H, W, 1, s);
   DVC_TRY(check_launch(c, "build_color_input"));
   return colorvid(c, tag, in0, out_ab, s);
 }
@@ -1738,58 +1772,71 @@ static int check_frame_args(dvc_ctx* c, int H, int W, float temperature, int K =
   return DVC_OK;
 }
 
-// B frames, each with its own L and previous Lab: against the one cached exemplar (K = 1) or frame b against slot b (K = B,
-// one clip per slot; workspaces of their own when K > 1, so alternating with the single-exemplar calls does not reallocate)
-static int colorize_frames_impl(dvc_ctx* c, const float* IA_l, const float* IA_last_lab, int B, int K, int H, int W,
-                                float temperature, float* out_ab, float* out_warp_lab, float* out_sim, cudaStream_t s) {
+// S frames, frame s with K[s] exemplar rows (row_table), each row with its own previous Lab: phase A once per frame at batch
+// S, the correlation and phase C over the R rows.  tagA names phase A's workspaces, tagC those of the rows.
+static int colorize_frames_impl(dvc_ctx* c, const char* tagA, const char* tagC, const float* IA_l, const float* IA_last_lab, int S,
+                                const int* K, int H, int W, float temperature, float* out_ab, float* out_warp_lab, float* out_sim,
+                                cudaStream_t s) {
   CUDA_TRY(c, cudaSetDevice(c->device));
-  const std::string tag = K > 1 ? "frs" : "fr";
+  PlaneSrc src;
+  const int R = row_table(S, K, &src);
   const int h = H / 4, w = W / 4, N = h * w;
+  const std::string tc = tagC;
   void *yrows, *simrows;
-  DVC_TRY(get_raw(c, tag + ".yrows", (size_t)B * N * 16, &yrows, s));
-  DVC_TRY(get_raw(c, tag + ".simrows", (size_t)B * N * 4, &simrows, s));
-  DVC_TRY(frames_phaseA(c, tag, IA_l, B, H, W, temperature, (float*)yrows, (float*)simrows, s, 0, nullptr, K));
+  DVC_TRY(get_raw(c, tc + ".yrows", (size_t)R * N * 16, &yrows, s));
+  DVC_TRY(get_raw(c, tc + ".simrows", (size_t)R * N * 4, &simrows, s));
+  DVC_TRY(frames_phaseA(c, tagA, IA_l, S, R, src, H, W, temperature, (float*)yrows, (float*)simrows, s));
   if (out_warp_lab || out_sim) {
-    launch_rows_to_nchw_up4((float*)yrows, (float*)simrows, out_warp_lab, out_sim, B, h, w, s);
+    launch_rows_to_nchw_up4((float*)yrows, (float*)simrows, out_warp_lab, out_sim, R, h, w, s);
     DVC_TRY(check_launch(c, "rows_to_nchw_up4"));
   }
-  return frames_phaseC(c, tag, IA_l, (float*)yrows, (float*)simrows, IA_last_lab, B, H, W, out_ab, s, (size_t)H * W);
+  return frames_phaseC(c, tc, IA_l, (float*)yrows, (float*)simrows, IA_last_lab, R, H, W, out_ab, s, src);
 }
 
 extern "C" int dvc_colorize_frames(dvc_ctx* c, const float* IA_l, const float* IA_last_lab, int B, int H, int W,
                                    float temperature, float* out_ab, float* out_warp_lab, float* out_sim, void* stream) {
   if (!c || !IA_l || !IA_last_lab || !out_ab || B < 1) return c ? fail(c, DVC_ERR_ARG, "colorize_frames: bad argument") : DVC_ERR_ARG;
   DVC_TRY(check_frame_args(c, H, W, temperature));
-  return colorize_frames_impl(c, IA_l, IA_last_lab, B, 1, H, W, temperature, out_ab, out_warp_lab, out_sim, (cudaStream_t)stream);
+  return colorize_frames_impl(c, "fr", "fr", IA_l, IA_last_lab, B, nullptr, H, W, temperature, out_ab, out_warp_lab, out_sim,
+                              (cudaStream_t)stream);
 }
 
+// Several clips: workspaces of their own when S > 1, so alternating with the single-exemplar calls does not reallocate
 extern "C" int dvc_colorize_frames_clips(dvc_ctx* c, const float* IA_l, const float* last_lab, int S, int H, int W, float temperature,
                                          float* out_ab, float* out_warp_lab, float* out_sim, void* stream) {
   if (!c || !IA_l || !last_lab || !out_ab) return c ? fail(c, DVC_ERR_ARG, "colorize_frames_clips: bad argument") : DVC_ERR_ARG;
   if (S < 1 || S > 8) return fail(c, DVC_ERR_ARG, "colorize_frames_clips: S must be in [1, 8]");
   DVC_TRY(check_frame_args(c, H, W, temperature, S));
-  return colorize_frames_impl(c, IA_l, last_lab, S, S, H, W, temperature, out_ab, out_warp_lab, out_sim, (cudaStream_t)stream);
+  const char* tag = S > 1 ? "frs" : "fr";
+  return colorize_frames_impl(c, tag, tag, IA_l, last_lab, S, nullptr, H, W, temperature, out_ab, out_warp_lab, out_sim,
+                              (cudaStream_t)stream);
 }
 
 // One frame against the K cached exemplars: phase A once at B = 1, the correlation against the K slots, phase C at
-// B = K with the frame's L shared by the K batches.
+// B = K with the frame's L shared by the K rows.
 extern "C" int dvc_colorize_frames_exemplars(dvc_ctx* c, const float* IA_l, const float* last_lab, int K, int H, int W,
                                              float temperature, float* out_ab, float* out_warp_lab, float* out_sim, void* stream) {
   if (!c || !IA_l || !last_lab || !out_ab) return c ? fail(c, DVC_ERR_ARG, "colorize_frames_exemplars: bad argument") : DVC_ERR_ARG;
   if (K < 1 || K > 8) return fail(c, DVC_ERR_ARG, "colorize_frames_exemplars: K must be in [1, 8]");
   DVC_TRY(check_frame_args(c, H, W, temperature, K));
-  cudaStream_t s = (cudaStream_t)stream;
-  CUDA_TRY(c, cudaSetDevice(c->device));
-  const int h = H / 4, w = W / 4, N = h * w;
-  void *yrows, *simrows;
-  DVC_TRY(get_raw(c, "frx.yrows", (size_t)K * N * 16, &yrows, s));
-  DVC_TRY(get_raw(c, "frx.simrows", (size_t)K * N * 4, &simrows, s));
-  DVC_TRY(frames_phaseA(c, "fr", IA_l, 1, H, W, temperature, (float*)yrows, (float*)simrows, s, 0, nullptr, K));
-  if (out_warp_lab || out_sim) {
-    launch_rows_to_nchw_up4((float*)yrows, (float*)simrows, out_warp_lab, out_sim, K, h, w, s);
-    DVC_TRY(check_launch(c, "rows_to_nchw_up4"));
-  }
-  return frames_phaseC(c, "frx", IA_l, (float*)yrows, (float*)simrows, last_lab, K, H, W, out_ab, s, 0);
+  return colorize_frames_impl(c, "fr", "frx", IA_l, last_lab, 1, &K, H, W, temperature, out_ab, out_warp_lab, out_sim,
+                              (cudaStream_t)stream);
+}
+
+// Frame s of S clips against the K[s] exemplar slots of clip s: phase A at batch S, the correlation and phase C over the
+// R = sum K[s] rows.  Every K[s] = 1 is dvc_colorize_frames_clips, S = 1 dvc_colorize_frames_exemplars.
+extern "C" int dvc_colorize_frames_clips_exemplars(dvc_ctx* c, const float* IA_l, const float* last_lab, int S, const int* K, int H,
+                                                   int W, float temperature, float* out_ab, float* out_warp_lab, float* out_sim,
+                                                   void* stream) {
+  const char* what = "colorize_frames_clips_exemplars";
+  if (!c || !IA_l || !last_lab || !out_ab) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
+  DVC_TRY(check_counts(c, what, S, K));
+  PlaneSrc src;
+  const int R = row_table(S, K, &src);
+  DVC_TRY(check_frame_args(c, H, W, temperature, R));
+  const char* tagA = S > 1 ? "frs" : "fr";
+  const char* tagC = R == S ? tagA : (S > 1 ? "frsx" : "frx");
+  return colorize_frames_impl(c, tagA, tagC, IA_l, last_lab, S, K, H, W, temperature, out_ab, out_warp_lab, out_sim, (cudaStream_t)stream);
 }
 
 static int clip_streams(dvc_ctx* c) {
@@ -1841,13 +1888,13 @@ static void fgs_lut(float sigma_color, float lut[256]) {
 }
 
 // num_iter FGS iterations (a horizontal and a vertical sweep each) over `planes` planes in place, lambda attenuated per
-// iteration; plane p takes the coefficients of guide p / planes_per_guide
-static void fgs_sweeps(float* planes_data, const float* Ch, const float* Cv, float* D, int planes, int planes_per_guide, int H, int W,
+// iteration; plane p takes the coefficients of guide gsrc.at(p / 2)
+static void fgs_sweeps(float* planes_data, const float* Ch, const float* Cv, float* D, int planes, const PlaneSrc& gsrc, int H, int W,
                        float lambda, float lambda_attenuation, int num_iter, cudaStream_t s) {
   float lam = lambda;
   for (int n = 0; n < num_iter; ++n) {
-    launch_fgs_horizontal(planes_data, Ch, D, planes, planes_per_guide, H, W, lam, s);
-    launch_fgs_vertical(planes_data, Cv, D, planes, planes_per_guide, H, W, lam, s);
+    launch_fgs_horizontal(planes_data, Ch, D, planes, gsrc, H, W, lam, s);
+    launch_fgs_vertical(planes_data, Cv, D, planes, gsrc, H, W, lam, s);
     lam *= lambda_attenuation;
   }
 }
@@ -1866,8 +1913,7 @@ static void rgb_from_xyz(double inv[9]) {
 // Ring slots (frame t uses slot t & 1 or t & 3) guarded by events of the frame that last used the slot; the kernels of one
 // stage run in order on one stream, so the stage's scratch buffers (fp64 resize planes, crop, FGS Ch / Cv / D, up-sampled
 // ab) exist once.  Nothing depends on F.
-// One frame source: dvc_colorize_video_rgb8 has one (its frames feed all K exemplars' recurrences), dvc_colorize_videos_rgb8
-// one per clip (clip s feeds batch s of the clip loop).
+// One frame source per clip: clip s feeds the clip loop's rows of clip s (one row per exemplar of that clip).
 struct VideoSrc {
   const unsigned char* frames = nullptr;  // [F][Hs][Ws][3], host (pinned) or device
   int Hs = 0, Ws = 0, Hr = 0, Wr = 0, oy = 0, ox = 0;
@@ -1881,8 +1927,8 @@ struct VideoIO {
   int Ho = 0, Wo = 0;
   bool wls = false;
   float lambda = 0.f, sigma = 0.f;
-  unsigned char* out = nullptr;  // [K or S][F][Ho][Wo][3], host (pinned) or device
-  float* last_out = nullptr;     // [K or S][3][Ho/2][Wo/2] or nullptr
+  unsigned char* out = nullptr;  // [R][F][Ho][Wo][3] (R rows of the clip loop), host (pinned) or device
+  float* last_out = nullptr;     // [R][3][Ho/2][Wo/2] or nullptr
   std::vector<double> taps;      // every source's [wy | wx | 1.0]: uploaded once per call
   float lut[256];
   // device workspaces
@@ -1906,7 +1952,7 @@ static int video_streams(dvc_ctx* c) {
 
 // workspaces, then the taps and the LUT on `s` (before the clip loop forks from it).  Several clips use workspaces of their
 // own, so alternating with dvc_colorize_video_rgb8 does not reallocate.
-static int video_prologue(dvc_ctx* c, VideoIO& v, int Kb, cudaStream_t s) {
+static int video_prologue(dvc_ctx* c, VideoIO& v, int R, cudaStream_t s) {
   const size_t S = v.clips.size(), hw = (size_t)v.Ho * v.Wo;
   const std::string pre = S > 1 ? "vids." : "vid.";
   auto raw = [&](const char* name, size_t bytes, auto** out) {
@@ -1921,14 +1967,14 @@ static int video_prologue(dvc_ctx* c, VideoIO& v, int Kb, cudaStream_t s) {
   DVC_TRY(raw("taps", v.taps.size() * 8, &v.dtaps));
   DVC_TRY(raw("crop", hw * 3, &v.crop));
   DVC_TRY(raw("L", 4 * S * hw * 4, &v.L));  // 4 slots, like the half-resolution L of the clip loop
-  DVC_TRY(raw("abL", (size_t)Kb * 2 * hw * 4, &v.abL));
-  DVC_TRY(raw("rgb", 2 * (size_t)Kb * hw * 3, &v.rgb));  // 2 slots
+  DVC_TRY(raw("abL", (size_t)R * 2 * hw * 4, &v.abL));
+  DVC_TRY(raw("rgb", 2 * (size_t)R * hw * 3, &v.rgb));  // 2 slots
   if (v.wls) {
     DVC_TRY(raw("guide", 4 * S * hw, &v.guide));  // 4 slots
     DVC_TRY(raw("lut", 256 * 4, &v.dlut));
     DVC_TRY(raw("Ch", S * hw * 4, &v.Ch));
     DVC_TRY(raw("Cv", S * hw * 4, &v.Cv));
-    DVC_TRY(raw("D", (size_t)Kb * 2 * hw * 4, &v.D));
+    DVC_TRY(raw("D", (size_t)R * 2 * hw * 4, &v.D));
     CUDA_TRY(c, cudaMemcpyAsync(v.dlut, v.lut, sizeof(v.lut), cudaMemcpyHostToDevice, s));
   }
   CUDA_TRY(c, cudaMemcpyAsync(v.dtaps, v.taps.data(), v.taps.size() * 8, cudaMemcpyHostToDevice, s));
@@ -1971,32 +2017,28 @@ static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
   return DVC_OK;
 }
 
-// frame t, once its ColorVidNet is done (evC[t & 3]): ab x2 * 1.25, FGS, Lab -> sRGB (stream P; records evP[t & 3], which
-// the reuse of the ab slot waits for) and the download (stream D; records evD[t & 3])
-static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int Kb, int F) {
+// frame t, once its ColorVidNet is done (evC[t & 3]): ab x2 * 1.25, FGS, Lab -> sRGB of the R rows, row r with the guide and
+// the full-resolution L of its clip src.at(r) (stream P; records evP[t & 3], which the reuse of the ab slot waits for) and the
+// download (stream D; records evD[t & 3])
+static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int R, const PlaneSrc& src, int F) {
   const size_t S = v.clips.size(), hw = (size_t)v.Ho * v.Wo;
   const float* Lfull = v.L + (size_t)(t & 3) * S * hw;
-  unsigned char* rgb = v.rgb + (size_t)(t & 1) * Kb * hw * 3;
+  unsigned char* rgb = v.rgb + (size_t)(t & 1) * R * hw * 3;
   CUDA_TRY(c, cudaStreamWaitEvent(c->sP, c->evC[t & 3], 0));
   if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sP, c->evD[(t - 2) & 3], 0));  // the rgb slot has been downloaded
-  launch_upsample2(abt, v.abL, Kb * 2, v.Ho / 2, v.Wo / 2, 1.25f, c->sP);  // test.py:100-102
-  if (v.wls) {  // test.py:105-112: one clip's a and b planes (of every exemplar) against that clip's guide, all in one launch
+  launch_upsample2(abt, v.abL, R * 2, v.Ho / 2, v.Wo / 2, 1.25f, c->sP);  // test.py:100-102
+  if (v.wls) {  // test.py:105-112: the a and b planes of every row against its clip's guide, all in one launch
     launch_fgs_weights(v.guide + (size_t)(t & 3) * S * hw, v.dlut, v.Ch, v.Cv, (int)S, v.Ho, v.Wo, c->sP);
-    fgs_sweeps(v.abL, v.Ch, v.Cv, v.D, Kb * 2, Kb * 2 / (int)S, v.Ho, v.Wo, v.lambda, 0.25f, 3, c->sP);
+    fgs_sweeps(v.abL, v.Ch, v.Cv, v.D, R * 2, src, v.Ho, v.Wo, v.lambda, 0.25f, 3, c->sP);
   }
   double inv[9];
   rgb_from_xyz(inv);
-  if (S > 1) {  // test.py:116-119: clip s's full-resolution L with its own ab
-    launch_lab_to_rgb8(Lfull, v.abL, rgb, (int)S, v.Ho, v.Wo, inv, c->sP);
-  } else {
-    for (int k = 0; k < Kb; ++k)  // the frame's full-resolution L for every exemplar
-      launch_lab_to_rgb8(Lfull, v.abL + (size_t)k * 2 * hw, rgb + (size_t)k * hw * 3, 1, v.Ho, v.Wo, inv, c->sP);
-  }
+  launch_lab_to_rgb8(Lfull, src, v.abL, rgb, R, v.Ho, v.Wo, inv, c->sP);  // test.py:116-119
   DVC_TRY(check_launch(c, "video post-processing"));
   CUDA_TRY(c, cudaEventRecord(c->evP[t & 3], c->sP));
   CUDA_TRY(c, cudaStreamWaitEvent(c->sD, c->evP[t & 3], 0));
-  for (int k = 0; k < Kb; ++k)
-    CUDA_TRY(c, cudaMemcpyAsync(v.out + ((size_t)k * F + t) * hw * 3, rgb + (size_t)k * hw * 3, hw * 3, cudaMemcpyDefault, c->sD));
+  for (int r = 0; r < R; ++r)
+    CUDA_TRY(c, cudaMemcpyAsync(v.out + ((size_t)r * F + t) * hw * 3, rgb + (size_t)r * hw * 3, hw * 3, cudaMemcpyDefault, c->sD));
   CUDA_TRY(c, cudaEventRecord(c->evD[t & 3], c->sD));
   return DVC_OK;
 }
@@ -2006,24 +2048,23 @@ static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int
 // partial waves of either leave SMs idle that the other fills.  Uploads of L (up to four frames ahead) and downloads
 // of ab run on two copy streams so that neither compute stream ever waits for PCIe.  L / ab may be host (pinned) or
 // device memory.
-// K = 0: dvc_colorize_clip (one exemplar); K >= 1: dvc_colorize_clip_exemplars, K recurrences sharing the luminance
-// sequence -- phase A once per frame against the K slots, phase C at batch K, and ab of exemplar k, frame t at
-// ab_out + (k F + t) 2 H W.  The multi-exemplar workspaces have tags of their own, so alternating does not reallocate.
-// S >= 1 (K = 0): dvc_colorize_clips, S clips, clip s against slot s -- L_in [S][F][H][W], phase A at batch S with frame s
-// against slot s, phase C at batch S with clip s's own L, ab of clip s at ab_out + (s F + t) 2 H W; several clips have
-// workspaces of their own too.  S = 0: not a several-clip call (one frame source).
+// S clips (L_in [S][F][H][W]) with K[s] exemplar rows each (row_table; K == nullptr: one row per clip), R rows in all: phase
+// A once per frame of every clip at batch S, the correlation of row r against exemplar slot r with clip src.at(r)'s query
+// set, phase C and make_last at batch R with each row's own recurrence last_r = cat(L_{src.at(r), t}, ab_{r, t}) (test.py:96),
+// and ab of row r, frame t at ab_out + (r F + t) 2 H W.  S = 0: dvc_colorize_clip (one clip, one row, and a multi-slot cache
+// refused).  S = 1, K = (K): dvc_colorize_clip_exemplars.  K == nullptr, S >= 1: dvc_colorize_clips.  Several clips, and
+// several exemplars per clip, use workspaces of their own, so alternating between the calls does not reallocate.
 // v != nullptr (dvc_colorize_video(s)_rgb8): frame t's L comes from video_ingest instead of L_in, and video_post replaces the
 // download of ab; the recurrence state after the last frame goes to v->last_out.
 static int colorize_clip_impl(dvc_ctx* c, const char* what, const float* L_in, int F, int H, int W, float temperature,
-                              const float* first_last, int K, int S, float* ab_out, void* stream, VideoIO* v = nullptr) {
+                              const float* first_last, int S, const int* K, float* ab_out, void* stream, VideoIO* v = nullptr) {
   if (!c || (!v && (!L_in || !ab_out)) || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
-  if (K < 0 || K > 8) return fail(c, DVC_ERR_ARG, std::string(what) + ": K must be in [1, 8]");
-  if (S < 0 || S > 8 || (K && S)) return fail(c, DVC_ERR_ARG, std::string(what) + ": S must be in [1, 8], without K exemplars");
-  DVC_TRY(check_frame_args(c, H, W, temperature, K ? K : S));
-  const int nsrc = S ? S : 1;    // frame sources: batch of phase A
-  const int Kb = K ? K : nsrc;   // batch of phase C
+  const int nsrc = S ? S : 1;  // frame sources: batch of phase A
+  PlaneSrc src;
+  const int R = row_table(nsrc, K, &src);  // batch of the correlation and phase C
+  DVC_TRY(check_frame_args(c, H, W, temperature, S ? R : 0));
   const bool clips = nsrc > 1;
-  const std::string tag = K ? "clipx" : (clips ? "clips" : "clip");
+  const std::string tag = std::string(clips ? "clips" : "clip") + (K ? "x" : "");
   cudaStream_t s = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->device));
   DVC_TRY(clip_streams(c));
@@ -2032,18 +2073,18 @@ static int colorize_clip_impl(dvc_ctx* c, const char* what, const float* L_in, i
   const int N = (H / 4) * (W / 4);
   void *dL, *dlast, *dab, *yrows, *simrows;
   DVC_TRY(get_raw(c, clips ? "clips.L" : "clip.L", 4 * (size_t)nsrc * hw * 4, &dL, s));   // 4 slots of nsrc planes
-  DVC_TRY(get_raw(c, tag + ".last", Kb * 3 * hw * 4, &dlast, s));
-  DVC_TRY(get_raw(c, tag + ".ab", 2 * Kb * 2 * hw * 4, &dab, s));  // 2 slots
-  DVC_TRY(get_raw(c, tag + ".yrows", (size_t)4 * Kb * N * 16, &yrows, s));  // 4 slots: phase A may run up to 3 frames ahead
-  DVC_TRY(get_raw(c, tag + ".simrows", (size_t)4 * Kb * N * 4, &simrows, s));
+  DVC_TRY(get_raw(c, tag + ".last", R * 3 * hw * 4, &dlast, s));
+  DVC_TRY(get_raw(c, tag + ".ab", 2 * R * 2 * hw * 4, &dab, s));  // 2 slots
+  DVC_TRY(get_raw(c, tag + ".yrows", (size_t)4 * R * N * 16, &yrows, s));  // 4 slots: phase A may run up to 3 frames ahead
+  DVC_TRY(get_raw(c, tag + ".simrows", (size_t)4 * R * N * 4, &simrows, s));
   const bool two_a = c->clip_astreams == 2;
   // the second phase-A stream has its own correlation workspace (sized like the first at dvc_set_exemplar time)
-  if (two_a && corr_ws_reserve(&c->corr_ws2, Kb, Kb, N, N) != 0) return fail(c, DVC_ERR_CUDA, std::string(what) + ": correlation workspace allocation failed");
-  if (v) DVC_TRY(video_prologue(c, *v, Kb, s));
+  if (two_a && corr_ws_reserve(&c->corr_ws2, R, R, N, N) != 0) return fail(c, DVC_ERR_CUDA, std::string(what) + ": correlation workspace allocation failed");
+  if (v) DVC_TRY(video_prologue(c, *v, R, s));
   if (first_last)
-    CUDA_TRY(c, cudaMemcpyAsync(dlast, first_last, Kb * 3 * hw * 4, cudaMemcpyDefault, s));
+    CUDA_TRY(c, cudaMemcpyAsync(dlast, first_last, R * 3 * hw * 4, cudaMemcpyDefault, s));
   else
-    CUDA_TRY(c, cudaMemsetAsync(dlast, 0, Kb * 3 * hw * 4, s));  // test.py:80
+    CUDA_TRY(c, cudaMemsetAsync(dlast, 0, R * 3 * hw * 4, s));  // test.py:80
   // Every exit below goes through the join epilogue: an error in the middle of the loop must not return while copies
   // or kernels of earlier frames are still writing into ab_out / the slots (a retry would race with them).
   auto enqueue = [&]() -> int {
@@ -2060,9 +2101,9 @@ static int colorize_clip_impl(dvc_ctx* c, const char* what, const float* L_in, i
     for (int t = 0; t < F; ++t) {
       const int slot = t & 1;
       float* Lt = (float*)dL + (size_t)(t & 3) * nsrc * hw;
-      float* abt = (float*)dab + (size_t)slot * Kb * 2 * hw;
-      float* yr = (float*)yrows + (size_t)(t & 3) * Kb * N * 4;
-      float* sr = (float*)simrows + (size_t)(t & 3) * Kb * N;
+      float* abt = (float*)dab + (size_t)slot * R * 2 * hw;
+      float* yr = (float*)yrows + (size_t)(t & 3) * R * N * 4;
+      float* sr = (float*)simrows + (size_t)(t & 3) * R * N;
       const bool odd = two_a && (t & 1);
       cudaStream_t sAt = odd ? c->sA2 : c->sA;
       if (v) {
@@ -2079,29 +2120,29 @@ static int colorize_clip_impl(dvc_ctx* c, const char* what, const float* L_in, i
       CUDA_TRY(c, cudaStreamWaitEvent(sAt, c->evU[t & 3], 0));
       if (t >= 4) CUDA_TRY(c, cudaStreamWaitEvent(sAt, c->evC[(t - 4) & 3], 0));
       const char* tagA = clips ? (odd ? "clipsA2" : "clipsA") : (odd ? "clipA2" : "clipA");
-      DVC_TRY(frames_phaseA(c, tagA, Lt, nsrc, H, W, temperature, yr, sr, sAt, odd ? 2 : 0, odd ? &c->corr_ws2 : nullptr, Kb));
+      DVC_TRY(frames_phaseA(c, tagA, Lt, nsrc, R, src, H, W, temperature, yr, sr, sAt, odd ? 2 : 0, odd ? &c->corr_ws2 : nullptr));
       CUDA_TRY(c, cudaEventRecord(c->evA[t & 3], sAt));
-      // ---- stream C: the recurrent phase (the K recurrences read the frame's one L plane, clip s its own plane s) ----
+      // ---- stream C: the recurrent phase (row r reads the L plane of its clip src.at(r)) ----
       CUDA_TRY(c, cudaStreamWaitEvent(c->sC, c->evA[t & 3], 0));
       // the ab slot has been downloaded (video: post-processed)
       if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sC, (v ? c->evP : c->evD)[(t - 2) & 3], 0));
-      const size_t l_bstride = clips ? hw : 0;
-      DVC_TRY(frames_phaseC(c, K ? "clipCx" : (clips ? "clipCs" : "clipC"), Lt, yr, sr, (float*)dlast, Kb, H, W, abt, c->sC, l_bstride));
-      launch_make_last(Lt, l_bstride, abt, (float*)dlast, Kb, H, W, c->sC);  // test.py:96
+      const std::string tagC = std::string(clips ? "clipCs" : "clipC") + (K ? "x" : "");
+      DVC_TRY(frames_phaseC(c, tagC, Lt, yr, sr, (float*)dlast, R, H, W, abt, c->sC, src));
+      launch_make_last(Lt, src, abt, (float*)dlast, R, H, W, c->sC);  // test.py:96
       DVC_TRY(check_launch(c, "make_last"));
       CUDA_TRY(c, cudaEventRecord(c->evC[t & 3], c->sC));
       if (v) {
-        DVC_TRY(video_post(c, *v, t, abt, Kb, F));
+        DVC_TRY(video_post(c, *v, t, abt, R, src, F));
         continue;
       }
       // ---- download stream ----
       CUDA_TRY(c, cudaStreamWaitEvent(c->sD, c->evC[t & 3], 0));
-      for (int k = 0; k < Kb; ++k)
-        CUDA_TRY(c, cudaMemcpyAsync(ab_out + ((size_t)k * F + t) * 2 * hw, abt + (size_t)k * 2 * hw, 2 * hw * 4, cudaMemcpyDefault, c->sD));
+      for (int r = 0; r < R; ++r)
+        CUDA_TRY(c, cudaMemcpyAsync(ab_out + ((size_t)r * F + t) * 2 * hw, abt + (size_t)r * 2 * hw, 2 * hw * 4, cudaMemcpyDefault, c->sD));
       CUDA_TRY(c, cudaEventRecord(c->evD[t & 3], c->sD));
     }
     if (v && v->last_out)  // cat(L/2, ab) of the last frame: the next segment's first_last
-      CUDA_TRY(c, cudaMemcpyAsync(v->last_out, dlast, Kb * 3 * hw * 4, cudaMemcpyDefault, c->sC));
+      CUDA_TRY(c, cudaMemcpyAsync(v->last_out, dlast, R * 3 * hw * 4, cudaMemcpyDefault, c->sC));
     return DVC_OK;
   };
   const int rc = enqueue();
@@ -2134,19 +2175,26 @@ static int colorize_clip_impl(dvc_ctx* c, const char* what, const float* L_in, i
 
 extern "C" int dvc_colorize_clip(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature,
                                  const float* first_last, float* ab_out, void* stream) {
-  return colorize_clip_impl(c, "colorize_clip", L_in, F, H, W, temperature, first_last, 0, 0, ab_out, stream);
+  return colorize_clip_impl(c, "colorize_clip", L_in, F, H, W, temperature, first_last, 0, nullptr, ab_out, stream);
 }
 
 extern "C" int dvc_colorize_clip_exemplars(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature,
                                            const float* first_last, int K, float* ab_out, void* stream) {
   if (c && (K < 1 || K > 8)) return fail(c, DVC_ERR_ARG, "colorize_clip_exemplars: K must be in [1, 8]");
-  return colorize_clip_impl(c, "colorize_clip_exemplars", L_in, F, H, W, temperature, first_last, K, 0, ab_out, stream);
+  return colorize_clip_impl(c, "colorize_clip_exemplars", L_in, F, H, W, temperature, first_last, 1, &K, ab_out, stream);
 }
 
 extern "C" int dvc_colorize_clips(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature, const float* first_last,
                                   int S, float* ab_out, void* stream) {
   if (c && (S < 1 || S > 8)) return fail(c, DVC_ERR_ARG, "colorize_clips: S must be in [1, 8]");
-  return colorize_clip_impl(c, "colorize_clips", L_in, F, H, W, temperature, first_last, 0, S, ab_out, stream);
+  return colorize_clip_impl(c, "colorize_clips", L_in, F, H, W, temperature, first_last, S, nullptr, ab_out, stream);
+}
+
+extern "C" int dvc_colorize_clips_exemplars(dvc_ctx* c, const float* L_in, int F, int H, int W, float temperature,
+                                            const float* first_last, int S, const int* K, float* ab_out, void* stream) {
+  const char* what = "colorize_clips_exemplars";
+  if (c) DVC_TRY(check_counts(c, what, S, K));
+  return colorize_clip_impl(c, what, L_in, F, H, W, temperature, first_last, S, c ? counts_or_null(S, K) : nullptr, ab_out, stream);
 }
 
 // One frame source of the video calls: geometry g = (Hs, Ws, Hr, Wr, oy, ox) checked as dvc_colorize_video_rgb8 documents
@@ -2197,15 +2245,21 @@ extern "C" int dvc_colorize_video_rgb8(dvc_ctx* c, const unsigned char* frames, 
   DVC_TRY(video_finish(c, what, v, wls, wls_lambda, wls_sigma, out, last_lab_out));
   // one exemplar: the single-exemplar loop (and its workspaces), as dvc_colorize_clip
   const int K = c->ex_valid && c->ex_K > 1 ? c->ex_K : 0;
-  return colorize_clip_impl(c, what, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, K, 0, nullptr, stream, &v);
+  return colorize_clip_impl(c, what, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, K ? 1 : 0, K ? &K : nullptr, nullptr,
+                            stream, &v);
 }
 
-extern "C" int dvc_colorize_videos_rgb8(dvc_ctx* c, int S, const unsigned char* const* frames, int F, const int* geom, int Ho, int Wo,
-                                        float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
-                                        unsigned char* out, float* last_lab_out, void* stream) {
-  const char* what = "colorize_videos_rgb8";
+// S clips, clip s with K[s] exemplar rows (K == nullptr: one each), every clip with its own geometry
+static int videos_impl(dvc_ctx* c, const char* what, int S, const int* K, const unsigned char* const* frames, int F, const int* geom,
+                       int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
+                       unsigned char* out, float* last_lab_out, void* stream) {
   if (!c || !frames || !geom || !out || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
-  if (S < 1 || S > 8) return fail(c, DVC_ERR_ARG, std::string(what) + ": S must be in [1, 8]");
+  if (K) {
+    DVC_TRY(check_counts(c, what, S, K));
+    K = counts_or_null(S, K);
+  } else if (S < 1 || S > 8) {
+    return fail(c, DVC_ERR_ARG, std::string(what) + ": S must be in [1, 8]");
+  }
   VideoIO v;
   v.Ho = Ho, v.Wo = Wo;
   for (int s = 0; s < S; ++s) {
@@ -2213,7 +2267,22 @@ extern "C" int dvc_colorize_videos_rgb8(dvc_ctx* c, int S, const unsigned char* 
     DVC_TRY(video_add_source(c, what, v, frames[s], geom + 6 * s));
   }
   DVC_TRY(video_finish(c, what, v, wls, wls_lambda, wls_sigma, out, last_lab_out));
-  return colorize_clip_impl(c, what, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, 0, S, nullptr, stream, &v);
+  return colorize_clip_impl(c, what, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, S, K, nullptr, stream, &v);
+}
+
+extern "C" int dvc_colorize_videos_rgb8(dvc_ctx* c, int S, const unsigned char* const* frames, int F, const int* geom, int Ho, int Wo,
+                                        float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
+                                        unsigned char* out, float* last_lab_out, void* stream) {
+  return videos_impl(c, "colorize_videos_rgb8", S, nullptr, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda,
+                     wls_sigma, out, last_lab_out, stream);
+}
+
+extern "C" int dvc_colorize_videos_exemplars_rgb8(dvc_ctx* c, int S, const int* K, const unsigned char* const* frames, int F,
+                                                  const int* geom, int Ho, int Wo, float temperature, const float* first_last_lab, int wls,
+                                                  float wls_lambda, float wls_sigma, unsigned char* out, float* last_lab_out, void* stream) {
+  if (c && !K) return fail(c, DVC_ERR_ARG, "colorize_videos_exemplars_rgb8: K is null");
+  return videos_impl(c, "colorize_videos_exemplars_rgb8", S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda,
+                     wls_sigma, out, last_lab_out, stream);
 }
 
 // ---- pre / post-processing around the nets (SURVEY.md §8f row 1) -----------------------------------------
@@ -2239,7 +2308,7 @@ extern "C" int dvc_lab_to_rgb8(dvc_ctx* c, const float* dev_l, const float* dev_
   CUDA_TRY(c, cudaSetDevice(c->device));
   double inv[9];
   rgb_from_xyz(inv);
-  launch_lab_to_rgb8(dev_l, dev_ab, dev_rgb, B, H, W, inv, (cudaStream_t)stream);
+  launch_lab_to_rgb8(dev_l, PlaneSrc::identity(), dev_ab, dev_rgb, B, H, W, inv, (cudaStream_t)stream);
   return check_launch(c, "lab_to_rgb8");
 }
 
@@ -2314,7 +2383,7 @@ extern "C" int dvc_fgs_filter(dvc_ctx* c, const unsigned char* dev_guide, const 
   launch_fgs_weights(dev_guide, (const float*)lut, (float*)Ch, (float*)Cv, 1, H, W, s);
   DVC_TRY(check_launch(c, "fgs_weights"));
   if (dev_dst != dev_src) CUDA_TRY(c, cudaMemcpyAsync(dev_dst, dev_src, (size_t)planes * hw * 4, cudaMemcpyDeviceToDevice, s));
-  fgs_sweeps(dev_dst, (const float*)Ch, (const float*)Cv, (float*)D, planes, planes, H, W, lambda, lambda_attenuation, num_iter, s);
+  fgs_sweeps(dev_dst, (const float*)Ch, (const float*)Cv, (float*)D, planes, PlaneSrc::shared(), H, W, lambda, lambda_attenuation, num_iter, s);
   return check_launch(c, "fgs");
 }
 

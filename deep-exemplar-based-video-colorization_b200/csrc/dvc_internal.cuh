@@ -93,6 +93,25 @@ __device__ __forceinline__ unsigned char guide8_of_l(float l) {
 }
 #endif
 
+// Which input plane each batch of a kernel reads when the inputs come in another count than the batches (query sets, L
+// planes, WLS guides): batch b reads plane at(b) = src[b].  A table holds the 8 rows of the multi-clip, multi-exemplar
+// calls; the stand-alone entry points also run more batches, always with the identity or with one shared plane, and a
+// batch past the table continues the step of its last two entries (the identity stays the identity, a shared plane shared).
+// The entries are 4-bit fields of one word: a lookup is a shift, where an indexed array would be copied to local memory.
+struct PlaneSrc {
+  unsigned int bits;  // src[b] in bits 4b .. 4b + 3
+  __host__ __device__ __forceinline__ int src(int b) const { return (int)((bits >> (4 * b)) & 15u); }
+  __host__ __device__ __forceinline__ int at(int b) const { return b < 8 ? src(b) : src(7) + (b - 7) * (src(7) - src(6)); }
+  void set(int b, int plane) { bits = (bits & ~(15u << (4 * b))) | ((unsigned int)plane << (4 * b)); }
+  static constexpr PlaneSrc identity() { return {0x76543210u}; }
+  static constexpr PlaneSrc shared() { return {0u}; }
+  int count(int B) const {  // planes the first B batches read: 1 + the largest index
+    int n = 0;
+    for (int b = 0; b < B; ++b) n = at(b) + 1 > n ? at(b) + 1 : n;
+    return n;
+  }
+};
+
 struct Act {
   float* d = nullptr;   // pixel (b=0, yp=0, xp=0), channel 0; the hi plane when lo != nullptr
   float* lo = nullptr;  // lo plane of a tf32 hi/lo split activation (value = hi + lo), same geometry
@@ -207,15 +226,15 @@ void launch_pack_v4(const float* src3, float* dst4, size_t n, cudaStream_t s);
 // y rows [B][N][4], sim rows [B][N] at h x w -> nearest x4 NCHW (NonlocalNet.py:499-500)
 void launch_rows_to_nchw_up4(const float* yrows, const float* simrows, float* y, float* sim, int B, int h, int w,
                              cudaStream_t s);
-// ColorVidNet input (FrameColor.py:64): [L, warped a, warped b, sim, last L, last a, last b, 0].  l_bstride: floats
-// between the L planes of consecutive batches (H * W, or 0: one luminance plane shared by every batch)
-void launch_build_color_input(const float* IA_l, size_t l_bstride, const float* yrows, const float* simrows,
+// ColorVidNet input (FrameColor.py:64): [L, warped a, warped b, sim, last L, last a, last b, 0].  Batch b reads the
+// luminance plane lsrc.at(b) of IA_l [*][H][W]
+void launch_build_color_input(const float* IA_l, const PlaneSrc& lsrc, const float* yrows, const float* simrows,
                               const float* last_lab, float* dst, int B, int H, int W, int P, cudaStream_t s);
 // conv10_ab (1x1, 128 -> 2) + tanh * 128 (ColorVidNet.py:143-144) -> NCHW [B][2][H][W]
 void launch_final_ab(const float* x, int H, int W, int P, int C, const float* w /*[2][C]*/, const float* bias,
                      float* out, int B, cudaStream_t s);
-// next frame's "last" = cat(L, ab) (test.py:96); l_bstride as for launch_build_color_input
-void launch_make_last(const float* IA_l, size_t l_bstride, const float* ab, float* last, int B, int H, int W, cudaStream_t s);
+// next frame's "last" = cat(L, ab) (test.py:96); lsrc as for launch_build_color_input
+void launch_make_last(const float* IA_l, const PlaneSrc& lsrc, const float* ab, float* last, int B, int H, int W, cudaStream_t s);
 
 // ---- correlation + softmax + warp (K7) ----------------------------------------------------------
 // Peer outputs of a query-row-sharded correlation (SURVEY.md 8e, config 4): the rank that owns query rows
@@ -229,13 +248,14 @@ struct CorrPeers {
 };
 
 struct CorrParams {
-  const float* theta;  // [B][NA][C]  (position-major, channels contiguous); [1][NA][C] when theta_shared
+  const float* theta;  // [qsrc.count(B)][NA][C]  (position-major, channels contiguous)
   const float* phi;    // [Bphi][NB][C]
   const float* V;      // [Bphi][NB][4] = (L, a, b, 1)
   int B, Bphi, NA, NB, C;
-  // one query set for every batch (query batch stride 0): batch b is that frame against reference set b (Bphi == B),
-  // e.g. one frame against K exemplars, without K copies of theta or of its operand planes
-  bool theta_shared = false;
+  // batch b correlates query set qsrc.at(b) with reference set b (or 0 when Bphi == 1): the identity pairs them, one
+  // shared set puts one frame against K exemplars, and a general table puts clip src[r] against exemplar row r -- without
+  // copies of theta or of its operand planes
+  PlaneSrc qsrc = PlaneSrc::identity();
   float temperature;
   float* y;     // [B][NA][4]
   float* sim;   // [B][NA]
@@ -261,16 +281,18 @@ void launch_resize_half(const float* src, float* dst, int planes, int H, int W, 
 void launch_upsample2(const float* src, float* dst, int planes, int h, int w, float scale, cudaStream_t s);
 // sRGB uint8 HWC -> centred Lab NCHW fp32 (skimage.color.rgb2lab semantics in float64, then L - 50)
 void launch_rgb8_to_lab(const unsigned char* rgb, float* lab, int B, int H, int W, cudaStream_t s);
-// Lab -> sRGB uint8 HWC in float64 (skimage.color.lab2rgb semantics); rgb_from_xyz: row-major 3x3
-void launch_lab_to_rgb8(const float* l, const float* ab, unsigned char* rgb, int B, int H, int W, const double* rgb_from_xyz,
-                        cudaStream_t s);
+// Lab -> sRGB uint8 HWC in float64 (skimage.color.lab2rgb semantics); batch b reads L plane lsrc.at(b) of l [*][H][W] and
+// its own ab [B][2][H][W]; rgb_from_xyz: row-major 3x3
+void launch_lab_to_rgb8(const float* l, const PlaneSrc& lsrc, const float* ab, unsigned char* rgb, int B, int H, int W,
+                        const double* rgb_from_xyz, cudaStream_t s);
 
 // Fast Global Smoother (test.py:105-112) and the CenterPad resize (util_distortion.py:217-258): prepost.cu
-// G guides [G][H][W] -> Ch / Cv [G][H][W]; the sweeps smooth plane p with the coefficients of guide p / planes_per_guide
+// G guides [G][H][W] -> Ch / Cv [G][H][W]; the sweeps smooth plane p with the coefficients of guide gsrc.at(p / 2) (the a and
+// b planes of one row share their guide)
 void launch_fgs_weights(const unsigned char* guide, const float* lut, float* Ch, float* Cv, int G, int H, int W, cudaStream_t s);
-void launch_fgs_horizontal(float* cur, const float* Ch, float* D, int planes, int planes_per_guide, int H, int W, float lam,
+void launch_fgs_horizontal(float* cur, const float* Ch, float* D, int planes, const PlaneSrc& gsrc, int H, int W, float lam,
                            cudaStream_t s);
-void launch_fgs_vertical(float* cur, const float* Cv, float* D, int planes, int planes_per_guide, int H, int W, float lam,
+void launch_fgs_vertical(float* cur, const float* Cv, float* D, int planes, const PlaneSrc& gsrc, int H, int W, float lam,
                          cudaStream_t s);
 void launch_l_to_guide8(const float* l, unsigned char* g, size_t n, cudaStream_t s);
 // video ingest: uint8 [H][W][3] (H, W even) -> centred L [H][W] (rgb8_to_lab's plane 0), its 1/2 resolution [H/2][W/2]

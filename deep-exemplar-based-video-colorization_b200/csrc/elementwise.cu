@@ -470,7 +470,7 @@ __global__ void __launch_bounds__(256) rows_to_nchw_up4_kernel(const float* __re
   }
 }
 
-__global__ void __launch_bounds__(256) build_color_input_kernel(const float* __restrict__ IA_l, size_t l_bstride,
+__global__ void __launch_bounds__(256) build_color_input_kernel(const float* __restrict__ IA_l, const PlaneSrc lsrc,
                                                                 const float* __restrict__ yrows,
                                                                 const float* __restrict__ simrows,
                                                                 const float* __restrict__ last, float* __restrict__ dst,
@@ -487,7 +487,7 @@ __global__ void __launch_bounds__(256) build_color_input_kernel(const float* __r
       const size_t q = (size_t)y * W + x;
       const int n = (y >> 2) * w + (x >> 2);
       const float4 yr = __ldg(reinterpret_cast<const float4*>(yrows + ((size_t)b * h * w + n) * 4));
-      o0.x = __ldg(IA_l + (size_t)b * l_bstride + q);
+      o0.x = __ldg(IA_l + (size_t)lsrc.at(b) * plane + q);
       o0.y = yr.y;  // warped a (channel 1 of the warped Lab, FrameColor.py:63)
       o0.z = yr.z;  // warped b
       o0.w = __ldg(simrows + (size_t)b * h * w + n);
@@ -534,11 +534,11 @@ __global__ void __launch_bounds__(256) final_ab_kernel(const float* __restrict__
   }
 }
 
-__global__ void __launch_bounds__(256) make_last_kernel(const float* __restrict__ IA_l, size_t l_bstride,
+__global__ void __launch_bounds__(256) make_last_kernel(const float* __restrict__ IA_l, const PlaneSrc lsrc,
                                                         const float* __restrict__ ab, float* __restrict__ last, int HW) {
   const int b = blockIdx.y;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x) {
-    last[((size_t)b * 3 + 0) * HW + i] = IA_l[(size_t)b * l_bstride + i];
+    last[((size_t)b * 3 + 0) * HW + i] = IA_l[(size_t)lsrc.at(b) * HW + i];
     last[((size_t)b * 3 + 1) * HW + i] = ab[((size_t)b * 2 + 0) * HW + i];
     last[((size_t)b * 3 + 2) * HW + i] = ab[((size_t)b * 2 + 1) * HW + i];
   }
@@ -694,10 +694,10 @@ void launch_rows_to_nchw_up4(const float* yrows, const float* simrows, float* y,
   launch_counter_add(1);
 }
 
-void launch_build_color_input(const float* IA_l, size_t l_bstride, const float* yrows, const float* simrows,
+void launch_build_color_input(const float* IA_l, const PlaneSrc& lsrc, const float* yrows, const float* simrows,
                               const float* last_lab, float* dst, int B, int H, int W, int P, cudaStream_t s) {
   dim3 grid(grid_for((long)(H + 2 * P) * (W + 2 * P), 256), B);
-  build_color_input_kernel<<<grid, 256, 0, s>>>(IA_l, l_bstride, yrows, simrows, last_lab, dst, H, W, P);
+  build_color_input_kernel<<<grid, 256, 0, s>>>(IA_l, lsrc, yrows, simrows, last_lab, dst, H, W, P);
   launch_counter_add(1);
 }
 
@@ -708,9 +708,9 @@ void launch_final_ab(const float* x, int H, int W, int P, int C, const float* w,
   launch_counter_add(1);
 }
 
-void launch_make_last(const float* IA_l, size_t l_bstride, const float* ab, float* last, int B, int H, int W, cudaStream_t s) {
+void launch_make_last(const float* IA_l, const PlaneSrc& lsrc, const float* ab, float* last, int B, int H, int W, cudaStream_t s) {
   dim3 grid(grid_for((long)H * W, 256), B);
-  make_last_kernel<<<grid, 256, 0, s>>>(IA_l, l_bstride, ab, last, H * W);
+  make_last_kernel<<<grid, 256, 0, s>>>(IA_l, lsrc, ab, last, H * W);
   launch_counter_add(1);
 }
 
@@ -719,11 +719,11 @@ struct Mat3 {
   double m[9];
 };
 // util.py:134-151 -> skimage.color.lab2rgb, all in float64 like the reference; one thread per pixel
-__global__ void __launch_bounds__(256) lab_to_rgb8_kernel(const float* __restrict__ l, const float* __restrict__ ab,
+__global__ void __launch_bounds__(256) lab_to_rgb8_kernel(const float* __restrict__ l, const PlaneSrc lsrc, const float* __restrict__ ab,
                                                           unsigned char* __restrict__ rgb, int HW, const Mat3 M) {
   const int b = blockIdx.y;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x) {
-    const double L = (double)l[(size_t)b * HW + i] + 50.0;  // l_norm = 1, l_mean = 50 (util.py:15-18)
+    const double L = (double)l[(size_t)lsrc.at(b) * HW + i] + 50.0;  // l_norm = 1, l_mean = 50 (util.py:15-18)
     const double A = (double)ab[((size_t)b * 2 + 0) * HW + i], Bq = (double)ab[((size_t)b * 2 + 1) * HW + i];
     double f[3];
     f[1] = (L + 16.0) / 116.0;
@@ -767,12 +767,12 @@ void launch_rgb8_to_lab(const unsigned char* rgb, float* lab, int B, int H, int 
   launch_counter_add(1);
 }
 
-void launch_lab_to_rgb8(const float* l, const float* ab, unsigned char* rgb, int B, int H, int W, const double* rgb_from_xyz,
-                        cudaStream_t s) {
+void launch_lab_to_rgb8(const float* l, const PlaneSrc& lsrc, const float* ab, unsigned char* rgb, int B, int H, int W,
+                        const double* rgb_from_xyz, cudaStream_t s) {
   Mat3 M;
   for (int i = 0; i < 9; ++i) M.m[i] = rgb_from_xyz[i];
   dim3 grid(grid_for((long)H * W, 256), B);
-  lab_to_rgb8_kernel<<<grid, 256, 0, s>>>(l, ab, rgb, H * W, M);
+  lab_to_rgb8_kernel<<<grid, 256, 0, s>>>(l, lsrc, ab, rgb, H * W, M);
   launch_counter_add(1);
 }
 

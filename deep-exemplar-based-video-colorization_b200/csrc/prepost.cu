@@ -44,16 +44,16 @@ __global__ void __launch_bounds__(256) fgs_weights_kernel(const unsigned char* _
 //   forward : denom_j = (1 - lam C_{j-1} - lam C_j) - lam C_{j-1} * D_{j-1};  D_j = lam C_j / denom_j;
 //             u_j = (u_j - lam C_{j-1} u_{j-1}) / denom_j
 //   backward: u_j = u_j - D_j u_{j+1}
-// Plane pl is smoothed with the coefficients of guide pl / planes_per_guide.
+// Plane pl is smoothed with the coefficients of guide gsrc.at(pl / 2): the a and b planes of one row share their guide.
 // Vertical sweep: thread = (plane, column), adjacent threads touch adjacent addresses (coalesced).
 __global__ void __launch_bounds__(128) fgs_vertical_kernel(float* __restrict__ cur, const float* __restrict__ Cv, float* __restrict__ D,
-                                                           int planes, int planes_per_guide, int H, int W, float lam) {
+                                                           int planes, const PlaneSrc gsrc, int H, int W, float lam) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= planes * W) return;
   const int pl = t / W, x = t - pl * W;
   float* u = cur + (size_t)pl * H * W + x;
   float* d = D + (size_t)pl * H * W + x;
-  const float* c = Cv + (size_t)(pl / planes_per_guide) * H * W + x;
+  const float* c = Cv + (size_t)gsrc.at(pl / 2) * H * W + x;
   float cprev = __fmul_rn(lam, c[0]);
   float denom = __fsub_rn(1.f, cprev);
   float dprev = __fdiv_rn(cprev, denom);
@@ -77,7 +77,7 @@ __global__ void __launch_bounds__(128) fgs_vertical_kernel(float* __restrict__ c
 // that are moved between global and shared memory with coalesced row accesses (a thread per row reading its own row
 // directly would touch one sector per element).
 __global__ void __launch_bounds__(32) fgs_horizontal_kernel(float* __restrict__ cur, const float* __restrict__ Ch, float* __restrict__ D,
-                                                            int planes, int planes_per_guide, int H, int W, float lam) {
+                                                            int planes, const PlaneSrc gsrc, int H, int W, float lam) {
   __shared__ float su[32][33], sc[32][33], sd[32][33];
   const int lane = threadIdx.x;
   const int groups = (H + 31) / 32;
@@ -85,7 +85,7 @@ __global__ void __launch_bounds__(32) fgs_horizontal_kernel(float* __restrict__ 
   const int nrows = min(32, H - r0);
   float* ub = cur + ((size_t)pl * H + r0) * W;
   float* db = D + ((size_t)pl * H + r0) * W;
-  const float* cb = Ch + ((size_t)(pl / planes_per_guide) * H + r0) * W;
+  const float* cb = Ch + ((size_t)gsrc.at(pl / 2) * H + r0) * W;
   float cprev = 0.f, dprev = 0.f, uprev = 0.f;
   for (int x0 = 0; x0 < W; x0 += 32) {
     const int nx = min(32, W - x0);
@@ -338,14 +338,14 @@ void launch_fgs_weights(const unsigned char* guide, const float* lut, float* Ch,
   fgs_weights_kernel<<<dim3(grid_for((size_t)H * W, 256), G), 256, 0, s>>>(guide, lut, Ch, Cv, H, W);
   launch_counter_add(1);
 }
-void launch_fgs_horizontal(float* cur, const float* Ch, float* D, int planes, int planes_per_guide, int H, int W, float lam,
+void launch_fgs_horizontal(float* cur, const float* Ch, float* D, int planes, const PlaneSrc& gsrc, int H, int W, float lam,
                            cudaStream_t s) {
-  fgs_horizontal_kernel<<<planes * ((H + 31) / 32), 32, 0, s>>>(cur, Ch, D, planes, planes_per_guide, H, W, lam);
+  fgs_horizontal_kernel<<<planes * ((H + 31) / 32), 32, 0, s>>>(cur, Ch, D, planes, gsrc, H, W, lam);
   launch_counter_add(1);
 }
-void launch_fgs_vertical(float* cur, const float* Cv, float* D, int planes, int planes_per_guide, int H, int W, float lam,
+void launch_fgs_vertical(float* cur, const float* Cv, float* D, int planes, const PlaneSrc& gsrc, int H, int W, float lam,
                          cudaStream_t s) {
-  fgs_vertical_kernel<<<(planes * W + 127) / 128, 128, 0, s>>>(cur, Cv, D, planes, planes_per_guide, H, W, lam);
+  fgs_vertical_kernel<<<(planes * W + 127) / 128, 128, 0, s>>>(cur, Cv, D, planes, gsrc, H, W, lam);
   launch_counter_add(1);
 }
 void launch_l_to_guide8(const float* l, unsigned char* g, size_t n, cudaStream_t s) {

@@ -30,7 +30,8 @@ EXPORTED = [
     "dvc_peer_buffer_create", "dvc_peer_buffer_open", "dvc_peer_buffer_close", "dvc_peer_buffer_destroy",
     "dvc_corr_set_peer_outputs", "dvc_set_exemplars", "dvc_colorize_frames_exemplars", "dvc_colorize_clip_exemplars",
     "dvc_corr_softmax_warp_exemplars", "dvc_colorize_video_rgb8", "dvc_colorize_frames_clips", "dvc_colorize_clips",
-    "dvc_colorize_videos_rgb8",
+    "dvc_colorize_videos_rgb8", "dvc_colorize_frames_clips_exemplars", "dvc_colorize_clips_exemplars",
+    "dvc_colorize_videos_exemplars_rgb8",
 ]
 
 _lib = None
@@ -85,6 +86,12 @@ def load_library():
         lib.dvc_colorize_clips.argtypes = [c_void, c_void, c_int, c_int, c_int, c_float, c_void, c_int, c_void, c_void]
         lib.dvc_colorize_videos_rgb8.argtypes = [c_void, c_int, P(c_void), c_int, P(c_int), c_int, c_int, c_float, c_void, c_int,
                                                  c_float, c_float, c_void, c_void, c_void]
+        lib.dvc_colorize_frames_clips_exemplars.argtypes = [c_void, c_void, c_void, c_int, P(c_int), c_int, c_int, c_float, c_void,
+                                                            c_void, c_void, c_void]
+        lib.dvc_colorize_clips_exemplars.argtypes = [c_void, c_void, c_int, c_int, c_int, c_float, c_void, c_int, P(c_int), c_void,
+                                                     c_void]
+        lib.dvc_colorize_videos_exemplars_rgb8.argtypes = [c_void, c_int, P(c_int), P(c_void), c_int, P(c_int), c_int, c_int, c_float,
+                                                           c_void, c_int, c_float, c_float, c_void, c_void, c_void]
         lib.dvc_exemplar_pack_size.argtypes = [c_void, c_int, c_int]
         lib.dvc_exemplar_pack_size.restype = c_i64
         lib.dvc_exemplar_export.argtypes = [c_void, c_void, c_i64, c_void]
@@ -491,6 +498,109 @@ class Context:
         rc = self.lib.dvc_colorize_videos_rgb8(self.h, S, ptrs, F_, g, Ho, Wo, float(temperature), _ptr(fl), 0 if wls is None else 1,
                                                lam, sigma, _ptr(out), _ptr(last), _stream(self.device))
         self._check(rc, "dvc_colorize_videos_rgb8")
+        return (out, last) if return_last else out
+
+    # ---- several clips in one pass, several exemplars each: K[s] rows per clip, R = sum(K) rows in all -------------------
+    # Row r is one (clip, exemplar) pair, the rows of clip s are contiguous and row r runs against cached exemplar slot r
+    # (set_exemplars with the R images in row order).  Every K[s] = 1 is the several-clip call, one clip the K-exemplar call.
+    @staticmethod
+    def _counts(K, S, what):
+        K = [int(k) for k in K]
+        if len(K) != S:
+            raise DvcError(f"{what}: K must give one exemplar count per clip ({S} clips, {len(K)} counts)")
+        return K, (ctypes.c_int * S)(*K)
+
+    def colorize_frames_clips_exemplars(self, IA_l, K, last, temperature=1e-10, want_warp=False):
+        """Frame s of IA_l [S,1,H,W] against the K[s] exemplar slots of clip s, last [R,3,H,W] -> ab [R,2,H,W]
+        (, warp [R,3,H,W], sim [R,1,H,W])."""
+        IA_l, last = _dev_f32(IA_l, "IA_l"), _dev_f32(last, "last")
+        S, c1, H, W = IA_l.shape
+        K, ck = self._counts(K, S, "colorize_frames_clips_exemplars")
+        R = sum(K)
+        if c1 != 1 or tuple(last.shape) != (R, 3, H, W):
+            raise DvcError("colorize_frames_clips_exemplars: IA_l must be [S,1,H,W] and last [R,3,H,W], R = sum(K)")
+        ab = torch.empty(R, 2, H, W, device=IA_l.device, dtype=torch.float32)
+        warp = torch.empty(R, 3, H, W, device=IA_l.device, dtype=torch.float32) if want_warp else None
+        sim = torch.empty(R, 1, H, W, device=IA_l.device, dtype=torch.float32) if want_warp else None
+        rc = self.lib.dvc_colorize_frames_clips_exemplars(self.h, _ptr(IA_l), _ptr(last), S, ck, H, W, float(temperature), _ptr(ab),
+                                                          _ptr(warp), _ptr(sim), _stream(IA_l.device))
+        self._check(rc, "dvc_colorize_frames_clips_exemplars")
+        return (ab, warp, sim) if want_warp else ab
+
+    def colorize_clips_exemplars(self, L, K, temperature=1e-10, first_last_lab=None, out=None):
+        """L [S,F,1,H,W] -> ab [R,F,2,H,W]: colorize_clips with K[s] exemplars for clip s, each row with its own recurrence.
+        first_last_lab: None (zeros) or [R,3,H,W].  L pinned on the host or on the device; `out` lives where L lives."""
+        if L.dtype != torch.float32 or L.dim() != 5 or L.shape[2] != 1:
+            raise DvcError("colorize_clips_exemplars takes a float32 [S,F,1,H,W] tensor")
+        L = L.contiguous()
+        S, F_, _, H, W = L.shape
+        K, ck = self._counts(K, S, "colorize_clips_exemplars")
+        R = sum(K)
+        if out is None:
+            out = torch.empty(R, F_, 2, H, W, dtype=torch.float32, device=L.device)
+            if not L.is_cuda:
+                out = out.pin_memory()
+        if out.is_cuda != L.is_cuda or not out.is_contiguous() or tuple(out.shape) != (R, F_, 2, H, W):
+            raise DvcError("colorize_clips_exemplars: `out` must be a contiguous [R,F,2,H,W] tensor on the same side as L")
+        fl = None
+        if first_last_lab is not None:
+            fl = first_last_lab.to(torch.float32).contiguous()
+            if tuple(fl.shape) != (R, 3, H, W):
+                raise DvcError("colorize_clips_exemplars: first_last_lab must be [R,3,H,W]")
+        rc = self.lib.dvc_colorize_clips_exemplars(self.h, _ptr(L), F_, H, W, float(temperature), _ptr(fl), S, ck, _ptr(out),
+                                                   _stream(self.device))
+        self._check(rc, "dvc_colorize_clips_exemplars")
+        return out
+
+    def colorize_videos_exemplars_rgb8(self, clips, K, size, temperature=1e-10, first_last_lab=None, wls=(500.0, 4.0), out=None,
+                                       return_last=False):
+        """colorize_videos_rgb8 with K[s] exemplars for clip s: clips is a list of S uint8 tensors [F,Hs_s,Ws_s,3] -> sRGB
+        uint8 [R,F,size[0],size[1],3], row r of clip s drawn with that clip's luminance and WLS guide.  first_last_lab / the
+        returned last state: [R,3,size[0]/2,size[1]/2]; the rest as colorize_videos_rgb8."""
+        from dvc.prepost import centerpad_geometry
+
+        clips = list(clips)
+        if not clips or not all(isinstance(f, torch.Tensor) and f.dtype == torch.uint8 and f.dim() == 4 and f.shape[3] == 3
+                                for f in clips):
+            raise DvcError("colorize_videos_exemplars_rgb8: expected a list of uint8 tensors [F,Hs,Ws,3]")
+        on_device = clips[0].is_cuda
+        if any(f.is_cuda != on_device for f in clips) or len({f.shape[0] for f in clips}) != 1:
+            raise DvcError("colorize_videos_exemplars_rgb8: the clips must have the same frame count and all live on the host or all "
+                           "on the device")
+        clips = [f.contiguous() for f in clips]
+        if not on_device:
+            clips = [f if f.is_pinned() else f.pin_memory() for f in clips]
+        S, F_ = len(clips), clips[0].shape[0]
+        K, ck = self._counts(K, S, "colorize_videos_exemplars_rgb8")
+        R = sum(K)
+        Ho, Wo = int(size[0]), int(size[1])
+        geom = []
+        for f in clips:
+            Hs, Ws = f.shape[1], f.shape[2]
+            geom += [Hs, Ws, *centerpad_geometry(Hs, Ws, (Ho, Wo))]
+
+        def host_or_device(shape, dtype):
+            t = torch.empty(*shape, dtype=dtype, device=clips[0].device)
+            return t if on_device else t.pin_memory()
+
+        if out is None:
+            out = host_or_device((R, F_, Ho, Wo, 3), torch.uint8)
+        if (out.is_cuda != on_device or out.dtype != torch.uint8 or not out.is_contiguous()
+                or tuple(out.shape) != (R, F_, Ho, Wo, 3)):
+            raise DvcError("colorize_videos_exemplars_rgb8: `out` must be a contiguous uint8 [R,F,H,W,3] tensor on the same side as "
+                           "the clips")
+        fl = None
+        if first_last_lab is not None:
+            fl = first_last_lab.to(torch.float32).contiguous()
+            if tuple(fl.shape) != (R, 3, Ho // 2, Wo // 2):
+                raise DvcError("colorize_videos_exemplars_rgb8: first_last_lab must be [R,3,H/2,W/2]")
+        last = host_or_device((R, 3, Ho // 2, Wo // 2), torch.float32) if return_last else None
+        lam, sigma = (0.0, 1.0) if wls is None else (float(wls[0]), float(wls[1]))
+        ptrs = (ctypes.c_void_p * S)(*[f.data_ptr() for f in clips])
+        g = (ctypes.c_int * (6 * S))(*geom)
+        rc = self.lib.dvc_colorize_videos_exemplars_rgb8(self.h, S, ck, ptrs, F_, g, Ho, Wo, float(temperature), _ptr(fl),
+                                                         0 if wls is None else 1, lam, sigma, _ptr(out), _ptr(last), _stream(self.device))
+        self._check(rc, "dvc_colorize_videos_exemplars_rgb8")
         return (out, last) if return_last else out
 
     # ---- pre / post-processing around the nets (test.py:58,71,100-102) ----------------------------------

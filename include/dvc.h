@@ -194,7 +194,8 @@ int dvc_colorize_video_rgb8(dvc_ctx* ctx, const unsigned char* frames, int F, in
  * stream in chunks and leave between calls.  S = 1 gives the bits of the single-exemplar calls; with S > 1 a clip's results
  * equal its solo run up to the InstanceNorm summation order and the device-derived fp16 scales that ColorVidNet shares
  * across its batch.  S outside [1, 8] is DVC_ERR_ARG; an S other than the cached exemplar count or a frame size other than
- * the exemplars' is DVC_ERR_SHAPE (so S clips with several exemplars each are refused).  A refused call launches nothing. */
+ * the exemplars' is DVC_ERR_SHAPE.  A refused call launches nothing.  Several exemplars per clip: the *_clips_exemplars
+ * entries below. */
 
 /* dvc_colorize_frames for S frames, frame s against slot s: dev_IA_l [S,1,H,W]; dev_last_lab [S,3,H,W]; dev_out_ab [S,2,H,W];
  * optional dev_out_warp_lab [S,3,H,W] and dev_out_sim [S,1,H,W] (may be NULL).  All device pointers. */
@@ -211,6 +212,34 @@ int dvc_colorize_clips(dvc_ctx* ctx, const float* L, int F, int H, int W, float 
 int dvc_colorize_videos_rgb8(dvc_ctx* ctx, int S, const unsigned char* const* frames, int F, const int* geom, int Ho, int Wo,
                              float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
                              unsigned char* out, float* last_lab_out, void* stream);
+
+/* ---- several clips in one pass, several exemplars each (the reference's data layout: a folder of reference images per
+ * clip, each colorizing the whole clip, test.py:168-181) -------------------------------------------------------------------
+ * Clip s has K[s] >= 1 exemplars; K points to the S per-clip counts.  A call works on R = K[0] + ... + K[S-1] rows: row r
+ * is one (clip, exemplar) pair, the rows of clip s are contiguous and in its exemplar order (clip s's first row is
+ * K[0] + ... + K[s-1]), and row r runs against cached exemplar slot r -- dvc_set_exemplars with the R images in row order.
+ * VGG19 and the WarpNet query side run once per clip frame at batch S; the correlation of row r pairs its clip's query set
+ * with slot r; ColorVidNet runs at batch R with each row's own recurrence last_r = cat(L_{clip of r},t, ab_r,t) (test.py:96).
+ * All tensors are row-major over the R rows, so the layouts contain the existing ones: with S = 1, [R,...] is the [K,...] of
+ * the *_exemplars calls, and with every K[s] = 1 the [S,...] of the several-clip calls -- whose bits these calls then give.
+ * S outside [1, 8], a null K, any K[s] < 1 or R > 8 is DVC_ERR_ARG; an R other than the cached exemplar count or a frame size
+ * other than the exemplars' is DVC_ERR_SHAPE.  A refused call launches nothing. */
+
+/* frame s of dev_IA_l [S,1,H,W] against the K[s] slots of clip s: dev_last_lab [R,3,H,W]; dev_out_ab [R,2,H,W]; optional
+ * dev_out_warp_lab [R,3,H,W] and dev_out_sim [R,1,H,W] (may be NULL).  All device pointers. */
+int dvc_colorize_frames_clips_exemplars(dvc_ctx* ctx, const float* dev_IA_l, const float* dev_last_lab, int S, const int* K, int H,
+                                        int W, float temperature, float* dev_out_ab, float* dev_out_warp_lab, float* dev_out_sim,
+                                        void* stream);
+/* dvc_colorize_clips with K[s] exemplars per clip: L [S,F,1,H,W]; first_last_lab NULL (zeros) or [R,3,H,W]; ab [R,F,2,H,W].
+ * Host (pinned) or device memory.  Synchronises `stream` before returning. */
+int dvc_colorize_clips_exemplars(dvc_ctx* ctx, const float* L, int F, int H, int W, float temperature, const float* first_last_lab,
+                                 int S, const int* K, float* ab, void* stream);
+/* dvc_colorize_videos_rgb8 with K[s] exemplars per clip: frames and geom as there; out [R,F,Ho,Wo,3]; first_last_lab and
+ * last_lab_out NULL or [R,3,Ho/2,Wo/2].  The post-processing of row r (WLS guide, full-resolution L) is its clip's.  Device
+ * memory does not depend on F.  Synchronises `stream` before returning. */
+int dvc_colorize_videos_exemplars_rgb8(dvc_ctx* ctx, int S, const int* K, const unsigned char* const* frames, int F, const int* geom,
+                                       int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda,
+                                       float wls_sigma, unsigned char* out, float* last_lab_out, void* stream);
 
 /* ---- pre / post-processing around the nets (SURVEY.md §8f row 1) ------------------------------ */
 

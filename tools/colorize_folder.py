@@ -15,11 +15,16 @@ by the chunk size, not by the clip length.  Consecutive frames of one source siz
 Several --ref images (test.py:168-181 colorizes the clip once per reference) take one pass: dvc_set_exemplars and the
 exemplar-independent half of every frame computed once; each exemplar's frames go to --out/<exemplar file name>/.
 
-Several --clip folders (at most 8) take one pass too, with exactly one --ref per clip: clip s against --ref s, its frames
-to --out/<clip folder name>/.  Every call (dvc_colorize_videos_rgb8) takes the same number of frames n from each clip that
-has frames left: n = min(--chunk, the run of frames of one source size each such clip has next).  When a clip runs out,
-it leaves: the others continue with dvc_set_exemplars of their references and their rows of the previous call's
-last_lab_out.  (Several clips with several references each are refused.)
+An entry of --ref may be a folder: its images, sorted by name (test.py's listing of ref_path), are that entry's exemplars.
+A single --clip with a --ref folder is the several-reference pass above.
+
+Several --clip folders (at most 8) take one pass too, with one --ref entry per clip, a file or a folder: clip s against the
+K_s exemplars of --ref s, at most 8 exemplars in all.  A clip with one exemplar writes to --out/<clip folder name>/, a clip
+with several to --out/<clip folder name>/<exemplar name>/.  Every call (dvc_colorize_videos_exemplars_rgb8 with the per-clip
+counts K_s, after dvc_set_exemplars of the clips' exemplars in clip order) takes the same number of frames n from each clip
+that has frames left: n = min(--chunk, the run of frames of one source size each such clip has next).  When a clip runs
+out, it leaves with its rows: the others continue with dvc_set_exemplars of their exemplars and their rows of the previous
+call's last_lab_out.
 
 What the reference does and this script does not: the AVI writer (folder2vid).  Image decode / encode stays on the host
 (PIL), as in the reference.  Without checkpoints (none ship with the reference tree) pass --seeded-weights to run the
@@ -87,9 +92,10 @@ def main():
                     help="folder(s) of frames (sorted by the digits in the file names, test.py:41); with several (at most 8), "
                          "one pass colorizes them all, each against its own --ref, into --out/<clip folder name>/")
     ap.add_argument("--ref", required=True, nargs="+",
-                    help="exemplar image(s); with several (at most 8), one pass colorizes the clip against each and writes "
-                         "--out/<exemplar name>/ (test.py:168-181 loops over a folder of references); with several --clip "
-                         "folders, exactly one per clip")
+                    help="exemplar image(s) or folder(s) of them (sorted by name); with several images (at most 8), one pass "
+                         "colorizes the clip against each and writes --out/<exemplar name>/ (test.py:168-181 loops over a folder "
+                         "of references); with several --clip folders, one entry (a file or a folder) per clip, and a clip with "
+                         "several exemplars writes --out/<clip folder name>/<exemplar name>/")
     ap.add_argument("--out", required=True)
     ap.add_argument("--vgg"), ap.add_argument("--warp"), ap.add_argument("--color")
     ap.add_argument("--seeded-weights", action="store_true")
@@ -110,8 +116,17 @@ def main():
     if S > 8:
         raise SystemExit("--clip: at most 8 folders in one pass")
     if S > 1 and len(args.ref) != S:
-        raise SystemExit("--ref: with several --clip folders, give exactly one exemplar per clip (several clips with several "
-                         "references each are not supported)")
+        raise SystemExit("--ref: with several --clip folders, give one entry (an image or a folder of images) per clip")
+    # each --ref entry: an image, or a folder whose images, sorted by name, are the entry's exemplars
+    ref_paths = [sorted(os.path.join(r, f) for f in os.listdir(r) if os.path.isfile(os.path.join(r, f))) if os.path.isdir(r) else [r]
+                 for r in args.ref]
+    if any(not p for p in ref_paths):
+        raise SystemExit("--ref: an empty folder")
+    if S == 1:
+        ref_paths = [[p for ps in ref_paths for p in ps]]  # one clip: every image is one of its exemplars
+    counts = [len(p) for p in ref_paths]
+    if sum(counts) > 8:
+        raise SystemExit(f"--ref: at most 8 exemplars in one pass, got {sum(counts)}")
 
     import dvc
     from dvc.synth import make_state_dict
@@ -131,29 +146,41 @@ def main():
     if H % 16 or W % 32:
         raise SystemExit("--image-size must have H % 16 == 0 and W % 32 == 0 (the networks run at half of it)")
     # test.py:44-46 + 57-66: CenterPad(image_size) + CenterCrop(image_size) of the exemplar(s), Lab, 1/2, features once
-    refs = torch.stack([ctx.centerpad_rgb8(torch.from_numpy(load_rgb8(r).copy()).cuda(), (H, W)) for r in args.ref])  # [K,H,W,3]
-    ref_lab = ctx.resize_half(ctx.rgb8_to_lab(refs))
-    if S > 1:  # clip s against exemplar s, every clip's recurrence in one pass
-        ctx.set_exemplars(ref_lab)
-        outs = [os.path.join(args.out, os.path.basename(os.path.normpath(d))) for d in args.clip]
-        if len(set(outs)) != len(outs):
-            raise SystemExit("--clip: the folder names must differ (they name the output folders)")
-    elif len(args.ref) == 1:
-        ctx.set_exemplar(ref_lab)
-        outs = [args.out]
+    def exemplars_lab(paths):  # [K,3,H/2,W/2]
+        refs = torch.stack([ctx.centerpad_rgb8(torch.from_numpy(load_rgb8(r).copy()).cuda(), (H, W)) for r in paths])  # [K,H,W,3]
+        return ctx.resize_half(ctx.rgb8_to_lab(refs))
+
+    ref_lab = [exemplars_lab(p) for p in ref_paths]  # per clip
+
+    def stem(path):
+        return os.path.splitext(os.path.basename(path))[0]
+
+    if S > 1:  # clip s against its K_s exemplars, every row's recurrence in one pass
+        ctx.set_exemplars(torch.cat(ref_lab))
+        outs = []  # per clip: the output folder of each of its exemplars
+        for d, paths in zip(args.clip, ref_paths):
+            base = os.path.join(args.out, os.path.basename(os.path.normpath(d)))
+            outs.append([base] if len(paths) == 1 else [os.path.join(base, stem(p)) for p in paths])
+        flat = [d for ds in outs for d in ds]
+        if len(set(flat)) != len(flat):
+            raise SystemExit("--clip / --ref: the output folders must differ (clip folder names, and the exemplar file names of a clip)")
+    elif counts[0] == 1:
+        ctx.set_exemplar(ref_lab[0])
+        outs = [[args.out]]
     else:  # every exemplar's recurrence in one pass over the clip
-        ctx.set_exemplars(ref_lab)
-        outs = [os.path.join(args.out, os.path.splitext(os.path.basename(r))[0]) for r in args.ref]
-        if len(set(outs)) != len(outs):
+        ctx.set_exemplars(ref_lab[0])
+        outs = [[os.path.join(args.out, stem(r)) for r in ref_paths[0]]]
+        if len(set(outs[0])) != len(outs[0]):
             raise SystemExit("--ref: the exemplar file names must differ (they name the output folders)")
-    for d in outs:
-        os.makedirs(d, exist_ok=True)
+    for ds in outs:
+        for d in ds:
+            os.makedirs(d, exist_ok=True)
     wls = None if args.no_wls else (args.lambda_value, args.sigma_color)
     C = args.chunk
 
     decode, encode = ThreadPoolExecutor(args.workers), ThreadPoolExecutor(args.workers)
     sources = [Source(d, decode, C) for d in args.clip]
-    active = list(range(S))  # clips with frames left; row j of a call's output and last_lab_out is clip active[j]
+    active = list(range(S))  # clips with frames left; a call's output and last_lab_out hold their rows, clip by clip
     ring_in = [[None] * S, [None] * S]  # pinned [C,Hs,Ws,3] frame chunks per clip
     ring_out = [None, None]  # pinned [rows,n,H,W,3] result chunks and the encodes still reading them
     writes = [[], []]
@@ -164,9 +191,11 @@ def main():
         if not keep:
             break
         if len(keep) < len(active):  # a clip ran out of frames: the others continue with their exemplars and states
-            active, runs = [active[j] for j in keep], [runs[j] for j in keep]
-            last = last[keep] if last is not None else None
-            ctx.set_exemplars(ref_lab[active])
+            stay = [active[j] for j in keep]
+            if last is not None:  # the rows of the clips that stay
+                last = last[[r for r, s in enumerate(s for s in active for _ in range(counts[s])) if s in stay]]
+            active, runs = stay, [runs[j] for j in keep]
+            ctx.set_exemplars(torch.cat([ref_lab[s] for s in active]))
         n, slot = min(runs), i & 1
         chunks = [sources[s].take(n) for s in active]
         for s, chunk in zip(active, chunks):
@@ -177,17 +206,18 @@ def main():
                 ring_in[slot][s][t].copy_(torch.from_numpy(img))
         for f in writes[slot]:  # the encodes of chunk i-2 still read this output slot
             f.result()
-        rows = len(outs) if S == 1 else len(active)
+        rows = sum(counts[s] for s in active)
         if ring_out[slot] is None or tuple(ring_out[slot].shape[:2]) != (rows, n):
             ring_out[slot] = torch.empty(rows, n, H, W, 3, dtype=torch.uint8).pin_memory()
         if S == 1:
             out, last = ctx.colorize_video_rgb8(ring_in[slot][0][:n], (H, W), args.temperature, first_last_lab=last, wls=wls,
                                                 out=ring_out[slot], return_last=True)
-            dests = [(outs[k], chunks[0]) for k in range(rows)]
+            dests = [(d, chunks[0]) for d in outs[0]]
         else:
-            out, last = ctx.colorize_videos_rgb8([ring_in[slot][s][:n] for s in active], (H, W), args.temperature,
-                                                 first_last_lab=last, wls=wls, out=ring_out[slot], return_last=True)
-            dests = [(outs[s], chunk) for s, chunk in zip(active, chunks)]
+            out, last = ctx.colorize_videos_exemplars_rgb8([ring_in[slot][s][:n] for s in active], [counts[s] for s in active], (H, W),
+                                                           args.temperature, first_last_lab=last, wls=wls, out=ring_out[slot],
+                                                           return_last=True)
+            dests = [(d, chunk) for s, chunk in zip(active, chunks) for d in outs[s]]
         arr = out.numpy()
         writes[slot] = [encode.submit(save_png, arr[r, t], os.path.join(d, os.path.splitext(name)[0] + ".png"))
                         for r, (d, chunk) in enumerate(dests) for t, (name, _) in enumerate(chunk)]
@@ -198,8 +228,9 @@ def main():
         for f in ws:
             f.result()
     decode.shutdown(), encode.shutdown()
-    for r, d in enumerate(outs):
-        print(f"{done[0 if S == 1 else r]} frames -> {d}")
+    for s, ds in enumerate(outs):
+        for d in ds:
+            print(f"{done[s]} frames -> {d}")
 
 
 if __name__ == "__main__":
