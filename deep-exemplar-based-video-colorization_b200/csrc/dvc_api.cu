@@ -1920,6 +1920,12 @@ struct VideoSrc {
   int ry = 0, rx = 0, ny = 0, nx = 0;
   size_t tap0 = 0;  // its [wy | wx | 1.0] in VideoIO::taps
   size_t src0 = 0;  // its frame in each of the two source slots
+  // source-resolution output (dvc_colorize_videos_source_rgb8): the footprint (y0, x0, h, w), the clip's rows of the clip loop,
+  // its [rows][F][h][w][3] output and its offsets in the source-resolution workspaces
+  int fp[4] = {0, 0, 0, 0};
+  int row0 = 0, rows = 1;
+  unsigned char* out = nullptr;
+  size_t sl0 = 0, sab0 = 0, srgb0 = 0;
 };
 struct VideoIO {
   std::vector<VideoSrc> clips;    // S sources
@@ -1931,10 +1937,17 @@ struct VideoIO {
   float* last_out = nullptr;     // [R][3][Ho/2][Wo/2] or nullptr
   std::vector<double> taps;      // every source's [wy | wx | 1.0]: uploaded once per call
   float lut[256];
+  // source-resolution output instead of `out`: the clips grouped by footprint size, pixels of one frame of every footprint, of
+  // every row's footprint, and the largest of one group (the FGS scratch is reused group after group)
+  bool source = false;
+  std::vector<std::vector<int>> groups;
+  size_t fp_sum = 0, fp_rows = 0, fp_max = 0, fp_rows_max = 0;
   // device workspaces
   unsigned char *src = nullptr, *crop = nullptr, *guide = nullptr, *rgb = nullptr;
   double *f0 = nullptr, *f1 = nullptr, *dtaps = nullptr;
   float *dlut = nullptr, *L = nullptr, *abL = nullptr, *Ch = nullptr, *Cv = nullptr, *D = nullptr;
+  float *sL = nullptr, *sab = nullptr;
+  unsigned char *sguide = nullptr, *srgb = nullptr;
 };
 
 static int video_streams(dvc_ctx* c) {
@@ -1968,14 +1981,28 @@ static int video_prologue(dvc_ctx* c, VideoIO& v, int R, cudaStream_t s) {
   DVC_TRY(raw("crop", hw * 3, &v.crop));
   DVC_TRY(raw("L", 4 * S * hw * 4, &v.L));  // 4 slots, like the half-resolution L of the clip loop
   DVC_TRY(raw("abL", (size_t)R * 2 * hw * 4, &v.abL));
-  DVC_TRY(raw("rgb", 2 * (size_t)R * hw * 3, &v.rgb));  // 2 slots
-  if (v.wls) {
-    DVC_TRY(raw("guide", 4 * S * hw, &v.guide));  // 4 slots
-    DVC_TRY(raw("lut", 256 * 4, &v.dlut));
-    DVC_TRY(raw("Ch", S * hw * 4, &v.Ch));
-    DVC_TRY(raw("Cv", S * hw * 4, &v.Cv));
-    DVC_TRY(raw("D", (size_t)R * 2 * hw * 4, &v.D));
-    CUDA_TRY(c, cudaMemcpyAsync(v.dlut, v.lut, sizeof(v.lut), cudaMemcpyHostToDevice, s));
+  if (v.source) {  // the source-resolution L and guide in 4 slots like v.L, the resampled ab, 2 rgb slots
+    DVC_TRY(raw("sL", 4 * v.fp_sum * 4, &v.sL));
+    DVC_TRY(raw("sab", v.fp_rows * 2 * 4, &v.sab));
+    DVC_TRY(raw("srgb", 2 * v.fp_rows * 3, &v.srgb));
+    if (v.wls) {
+      DVC_TRY(raw("sguide", 4 * v.fp_sum, &v.sguide));
+      DVC_TRY(raw("lut", 256 * 4, &v.dlut));
+      DVC_TRY(raw("sCh", v.fp_max * 4, &v.Ch));
+      DVC_TRY(raw("sCv", v.fp_max * 4, &v.Cv));
+      DVC_TRY(raw("sD", v.fp_rows_max * 2 * 4, &v.D));
+      CUDA_TRY(c, cudaMemcpyAsync(v.dlut, v.lut, sizeof(v.lut), cudaMemcpyHostToDevice, s));
+    }
+  } else {
+    DVC_TRY(raw("rgb", 2 * (size_t)R * hw * 3, &v.rgb));  // 2 slots
+    if (v.wls) {
+      DVC_TRY(raw("guide", 4 * S * hw, &v.guide));  // 4 slots
+      DVC_TRY(raw("lut", 256 * 4, &v.dlut));
+      DVC_TRY(raw("Ch", S * hw * 4, &v.Ch));
+      DVC_TRY(raw("Cv", S * hw * 4, &v.Cv));
+      DVC_TRY(raw("D", (size_t)R * 2 * hw * 4, &v.D));
+      CUDA_TRY(c, cudaMemcpyAsync(v.dlut, v.lut, sizeof(v.lut), cudaMemcpyHostToDevice, s));
+    }
   }
   CUDA_TRY(c, cudaMemcpyAsync(v.dtaps, v.taps.data(), v.taps.size() * 8, cudaMemcpyHostToDevice, s));
   return DVC_OK;
@@ -2010,11 +2037,43 @@ static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
       std::swap(cur, nxt);
     }
     launch_zoom_crop(cur, k.Hs, k.Ws, k.Hr, k.Wr, k.oy, k.ox, v.crop, v.Ho, v.Wo, c->sI);
-    launch_rgb8_to_l_half(v.crop, v.L + plane * hw, Lt + s * (hw / 4), v.wls ? v.guide + plane * hw : nullptr, v.Ho, v.Wo, c->sI);
+    launch_rgb8_to_l_half(v.crop, v.L + plane * hw, Lt + s * (hw / 4), v.wls && !v.source ? v.guide + plane * hw : nullptr, v.Ho, v.Wo,
+                          c->sI);
+    if (v.source) {  // the source frame's own L and guide over its footprint, while its upload slot is still held
+      const size_t sp = (size_t)(t & 3) * v.fp_sum + k.sl0;
+      launch_rgb8_to_l_guide(src + k.src0, k.Ws, k.fp[0], k.fp[1], k.fp[2], k.fp[3], v.sL + sp, v.wls ? v.sguide + sp : nullptr, c->sI);
+    }
   }
   DVC_TRY(check_launch(c, "video ingest"));
   CUDA_TRY(c, cudaEventRecord(c->evU[t & 3], c->sI));
   return DVC_OK;
+}
+
+// Source-resolution post-processing of frame t (stream s), after the window ab of all rows is in v.abL: per clip, its rows' ab
+// resampled onto its footprint (its own geometry); per group of clips with one footprint size, the FGS of the group's planes,
+// row j guided by the source frame of its clip, and Lab -> sRGB with that frame's own L -- one launch each per group
+// (1 + 6 + 1 with WLS), like the window-size post-processing per call.
+static void video_post_source(const VideoIO& v, int t, const double inv[9], cudaStream_t s) {
+  const size_t hw = (size_t)v.Ho * v.Wo, slot = (size_t)(t & 3) * v.fp_sum;
+  unsigned char* rgb = v.srgb + (size_t)(t & 1) * v.fp_rows * 3;
+  for (const auto& grp : v.groups) {
+    const VideoSrc& k0 = v.clips[grp[0]];
+    const int h = k0.fp[2], w = k0.fp[3];
+    PlaneSrc src = PlaneSrc::shared();  // row j of the group reads guide / L plane src[j]: its clip's place in the group
+    int rows = 0;
+    for (size_t i = 0; i < grp.size(); ++i) {
+      const VideoSrc& k = v.clips[grp[i]];
+      const int g[6] = {k.Hs, k.Ws, k.Hr, k.Wr, k.oy, k.ox};
+      launch_ab_to_source(v.abL + (size_t)k.row0 * 2 * hw, 2 * k.rows, v.Ho, v.Wo, g, k.fp, v.sab + k.sab0, s);
+      for (int r = 0; r < k.rows; ++r, ++rows) src.set(rows, (int)i);
+    }
+    float* ab = v.sab + k0.sab0;
+    if (v.wls) {
+      launch_fgs_weights(v.sguide + slot + k0.sl0, v.dlut, v.Ch, v.Cv, (int)grp.size(), h, w, s);
+      fgs_sweeps(ab, v.Ch, v.Cv, v.D, 2 * rows, src, h, w, v.lambda, 0.25f, 3, s);
+    }
+    launch_lab_to_rgb8(v.sL + slot + k0.sl0, src, ab, rgb + k0.srgb0, rows, h, w, inv, s);
+  }
 }
 
 // frame t, once its ColorVidNet is done (evC[t & 3]): ab x2 * 1.25, FGS, Lab -> sRGB of the R rows, row r with the guide and
@@ -2023,22 +2082,35 @@ static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
 static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int R, const PlaneSrc& src, int F) {
   const size_t S = v.clips.size(), hw = (size_t)v.Ho * v.Wo;
   const float* Lfull = v.L + (size_t)(t & 3) * S * hw;
-  unsigned char* rgb = v.rgb + (size_t)(t & 1) * R * hw * 3;
+  unsigned char* rgb = v.source ? nullptr : v.rgb + (size_t)(t & 1) * R * hw * 3;  // source output: video_post_source's slots
   CUDA_TRY(c, cudaStreamWaitEvent(c->sP, c->evC[t & 3], 0));
   if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sP, c->evD[(t - 2) & 3], 0));  // the rgb slot has been downloaded
   launch_upsample2(abt, v.abL, R * 2, v.Ho / 2, v.Wo / 2, 1.25f, c->sP);  // test.py:100-102
-  if (v.wls) {  // test.py:105-112: the a and b planes of every row against its clip's guide, all in one launch
-    launch_fgs_weights(v.guide + (size_t)(t & 3) * S * hw, v.dlut, v.Ch, v.Cv, (int)S, v.Ho, v.Wo, c->sP);
-    fgs_sweeps(v.abL, v.Ch, v.Cv, v.D, R * 2, src, v.Ho, v.Wo, v.lambda, 0.25f, 3, c->sP);
-  }
   double inv[9];
   rgb_from_xyz(inv);
-  launch_lab_to_rgb8(Lfull, src, v.abL, rgb, R, v.Ho, v.Wo, inv, c->sP);  // test.py:116-119
+  if (v.source) {  // the same recipe one step further, clip by clip at its footprint size
+    video_post_source(v, t, inv, c->sP);
+  } else {
+    if (v.wls) {  // test.py:105-112: the a and b planes of every row against its clip's guide, all in one launch
+      launch_fgs_weights(v.guide + (size_t)(t & 3) * S * hw, v.dlut, v.Ch, v.Cv, (int)S, v.Ho, v.Wo, c->sP);
+      fgs_sweeps(v.abL, v.Ch, v.Cv, v.D, R * 2, src, v.Ho, v.Wo, v.lambda, 0.25f, 3, c->sP);
+    }
+    launch_lab_to_rgb8(Lfull, src, v.abL, rgb, R, v.Ho, v.Wo, inv, c->sP);  // test.py:116-119
+  }
   DVC_TRY(check_launch(c, "video post-processing"));
   CUDA_TRY(c, cudaEventRecord(c->evP[t & 3], c->sP));
   CUDA_TRY(c, cudaStreamWaitEvent(c->sD, c->evP[t & 3], 0));
-  for (int r = 0; r < R; ++r)
-    CUDA_TRY(c, cudaMemcpyAsync(v.out + ((size_t)r * F + t) * hw * 3, rgb + (size_t)r * hw * 3, hw * 3, cudaMemcpyDefault, c->sD));
+  if (v.source) {
+    const unsigned char* srgb = v.srgb + (size_t)(t & 1) * v.fp_rows * 3;
+    for (const VideoSrc& k : v.clips) {
+      const size_t n3 = (size_t)k.fp[2] * k.fp[3] * 3;
+      for (int r = 0; r < k.rows; ++r)
+        CUDA_TRY(c, cudaMemcpyAsync(k.out + ((size_t)r * F + t) * n3, srgb + k.srgb0 + r * n3, n3, cudaMemcpyDefault, c->sD));
+    }
+  } else {
+    for (int r = 0; r < R; ++r)
+      CUDA_TRY(c, cudaMemcpyAsync(v.out + ((size_t)r * F + t) * hw * 3, rgb + (size_t)r * hw * 3, hw * 3, cudaMemcpyDefault, c->sD));
+  }
   CUDA_TRY(c, cudaEventRecord(c->evD[t & 3], c->sD));
   return DVC_OK;
 }
@@ -2222,6 +2294,61 @@ static int video_add_source(dvc_ctx* c, const char* what, VideoIO& v, const unsi
   return DVC_OK;
 }
 
+// The source pixels whose centres fall inside the window's extent [-0.5, Ho - 0.5] along one axis: ys iff
+// 2 oy Hs <= (2 ys + 1) Hr <= 2 (oy + Ho) Hs, in exact integer arithmetic.  A contiguous run (the middle term grows with ys).
+static void footprint_axis(long long Hs, long long Hr, long long oy, long long Ho, int* first, int* count) {
+  *first = 0, *count = 0;
+  for (long long ys = 0; ys < Hs; ++ys) {
+    const long long p = (2 * ys + 1) * Hr;
+    if (p < 2 * oy * Hs) continue;
+    if (p > 2 * (oy + Ho) * Hs) break;
+    if (!*count) *first = (int)ys;
+    ++*count;
+  }
+}
+
+extern "C" int dvc_source_footprint(int Hs, int Ws, int Hr, int Wr, int oy, int ox, int Ho, int Wo, int out[4]) {
+  if (!out || Hs < 1 || Ws < 1 || Hr < 1 || Wr < 1 || Ho < 1 || Wo < 1) return DVC_ERR_ARG;
+  int fp[4];
+  footprint_axis(Hs, Hr, oy, Ho, &fp[0], &fp[2]);
+  footprint_axis(Ws, Wr, ox, Wo, &fp[1], &fp[3]);
+  if (!fp[2] || !fp[3]) return DVC_ERR_SHAPE;  // no source pixel centre inside the window
+  for (int i = 0; i < 4; ++i) out[i] = fp[i];
+  return DVC_OK;
+}
+
+// Source-resolution output of the video call: clip s's footprint, its K[s] rows and its out[s]; the clips grouped by footprint
+// size, and the workspace offsets laid out group by group, so that a group's L / guide planes, ab rows and rgb rows are
+// contiguous and its FGS and Lab -> sRGB run as one launch each
+static int video_source_outputs(dvc_ctx* c, const char* what, VideoIO& v, const int* K, unsigned char* const* out) {
+  v.source = true;
+  int row0 = 0;
+  for (size_t s = 0; s < v.clips.size(); ++s) {
+    VideoSrc& k = v.clips[s];
+    if (!out[s]) return fail(c, DVC_ERR_ARG, std::string(what) + ": out[" + std::to_string(s) + "] is null");
+    if (dvc_source_footprint(k.Hs, k.Ws, k.Hr, k.Wr, k.oy, k.ox, v.Ho, v.Wo, k.fp) != DVC_OK)
+      return fail(c, DVC_ERR_SHAPE, std::string(what) + ": clip " + std::to_string(s) + " has no source pixel inside the window");
+    k.out = out[s], k.row0 = row0, k.rows = K[s];
+    row0 += K[s];
+    bool placed = false;
+    for (auto& g : v.groups)
+      if (v.clips[g[0]].fp[2] == k.fp[2] && v.clips[g[0]].fp[3] == k.fp[3]) g.push_back((int)s), placed = true;
+    if (!placed) v.groups.push_back({(int)s});
+  }
+  for (const auto& g : v.groups) {
+    size_t gpix = 0, grows = 0;
+    for (int s : g) {
+      VideoSrc& k = v.clips[s];
+      const size_t n = (size_t)k.fp[2] * k.fp[3];
+      k.sl0 = v.fp_sum, k.sab0 = 2 * v.fp_rows, k.srgb0 = 3 * v.fp_rows;
+      v.fp_sum += n, v.fp_rows += n * k.rows;
+      gpix += n, grows += n * k.rows;
+    }
+    v.fp_max = std::max(v.fp_max, gpix), v.fp_rows_max = std::max(v.fp_rows_max, grows);
+  }
+  return DVC_OK;
+}
+
 // the checks and settings the video calls share, after their sources: output size, WLS parameters, outputs
 static int video_finish(dvc_ctx* c, const char* what, VideoIO& v, int wls, float wls_lambda, float wls_sigma, unsigned char* out,
                         float* last_lab_out) {
@@ -2249,11 +2376,13 @@ extern "C" int dvc_colorize_video_rgb8(dvc_ctx* c, const unsigned char* frames, 
                             stream, &v);
 }
 
-// S clips, clip s with K[s] exemplar rows (K == nullptr: one each), every clip with its own geometry
+// S clips, clip s with K[s] exemplar rows (K == nullptr: one each), every clip with its own geometry.  The output is `out` at
+// the window size, or clip s's own source_out[s] at its footprint size (source_out != nullptr; K given then).
 static int videos_impl(dvc_ctx* c, const char* what, int S, const int* K, const unsigned char* const* frames, int F, const int* geom,
                        int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
-                       unsigned char* out, float* last_lab_out, void* stream) {
-  if (!c || !frames || !geom || !out || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
+                       unsigned char* out, float* last_lab_out, void* stream, unsigned char* const* source_out = nullptr) {
+  if (!c || !frames || !geom || (!out && !source_out) || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
+  const int* counts = K;
   if (K) {
     DVC_TRY(check_counts(c, what, S, K));
     K = counts_or_null(S, K);
@@ -2267,6 +2396,7 @@ static int videos_impl(dvc_ctx* c, const char* what, int S, const int* K, const 
     DVC_TRY(video_add_source(c, what, v, frames[s], geom + 6 * s));
   }
   DVC_TRY(video_finish(c, what, v, wls, wls_lambda, wls_sigma, out, last_lab_out));
+  if (source_out) DVC_TRY(video_source_outputs(c, what, v, counts, source_out));
   return colorize_clip_impl(c, what, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, S, K, nullptr, stream, &v);
 }
 
@@ -2283,6 +2413,29 @@ extern "C" int dvc_colorize_videos_exemplars_rgb8(dvc_ctx* c, int S, const int* 
   if (c && !K) return fail(c, DVC_ERR_ARG, "colorize_videos_exemplars_rgb8: K is null");
   return videos_impl(c, "colorize_videos_exemplars_rgb8", S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda,
                      wls_sigma, out, last_lab_out, stream);
+}
+
+extern "C" int dvc_colorize_videos_source_rgb8(dvc_ctx* c, int S, const int* K, const unsigned char* const* frames, int F,
+                                               const int* geom, int Ho, int Wo, float temperature, const float* first_last_lab, int wls,
+                                               float wls_lambda, float wls_sigma, unsigned char* const* out, float* last_lab_out,
+                                               void* stream) {
+  const char* what = "colorize_videos_source_rgb8";
+  if (c && !K) return fail(c, DVC_ERR_ARG, std::string(what) + ": K is null");
+  if (c && !out) return fail(c, DVC_ERR_ARG, std::string(what) + ": out is null");
+  return videos_impl(c, what, S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda, wls_sigma, nullptr,
+                     last_lab_out, stream, out);
+}
+
+extern "C" int dvc_ab_to_source(dvc_ctx* c, const float* dev_ab, int planes, int Ho, int Wo, int Hs, int Ws, int Hr, int Wr, int oy, int ox,
+                                float* dev_dst, void* stream) {
+  if (!c || !dev_ab || !dev_dst || planes < 1) return c ? fail(c, DVC_ERR_ARG, "ab_to_source: bad argument") : DVC_ERR_ARG;
+  int fp[4];
+  const int rc = dvc_source_footprint(Hs, Ws, Hr, Wr, oy, ox, Ho, Wo, fp);
+  if (rc != DVC_OK) return fail(c, rc, "ab_to_source: bad geometry (sizes >= 1, a source pixel inside the window)");
+  CUDA_TRY(c, cudaSetDevice(c->device));
+  const int g[6] = {Hs, Ws, Hr, Wr, oy, ox};
+  launch_ab_to_source(dev_ab, planes, Ho, Wo, g, fp, dev_dst, (cudaStream_t)stream);
+  return check_launch(c, "ab_to_source");
 }
 
 // ---- pre / post-processing around the nets (SURVEY.md §8f row 1) -----------------------------------------

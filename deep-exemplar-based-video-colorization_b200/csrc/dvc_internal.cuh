@@ -298,6 +298,12 @@ void launch_l_to_guide8(const float* l, unsigned char* g, size_t n, cudaStream_t
 // video ingest: uint8 [H][W][3] (H, W even) -> centred L [H][W] (rgb8_to_lab's plane 0), its 1/2 resolution [H/2][W/2]
 // (resize_half of that plane) and, when guide != nullptr, the WLS guide [H][W] (l_to_guide8 of the L plane)
 void launch_rgb8_to_l_half(const unsigned char* rgb, float* l, float* l_half, unsigned char* guide, int H, int W, cudaStream_t s);
+// source-resolution output of the video path: the footprint (y0, x0, h, w) of a uint8 frame [Hs][Ws][3] -> centred L [h][w]
+// (rgb8_to_lab's plane 0) and, when guide != nullptr, the WLS guide [h][w]
+void launch_rgb8_to_l_guide(const unsigned char* rgb, int Ws, int y0, int x0, int h, int w, float* l, unsigned char* guide, cudaStream_t s);
+// window ab [planes][Ho][Wo] -> bilinear on the footprint fp = (y0, x0, h, w) of the source grid of geometry g = (Hs, Ws, Hr, Wr,
+// oy, ox): dst [planes][h][w]
+void launch_ab_to_source(const float* ab, int planes, int Ho, int Wo, const int g[6], const int fp[4], float* dst, cudaStream_t s);
 void launch_gauss_axis_u8(const unsigned char* src, double* dst, const double* w, int radius, size_t n_outer, int len, int inner,
                           cudaStream_t s);
 void launch_gauss_axis_f64(const double* src, double* dst, const double* w, int radius, size_t n_outer, int len, int inner,

@@ -166,6 +166,48 @@ __global__ void __launch_bounds__(256) rgb8_to_l_half_kernel(const unsigned char
   }
 }
 
+// Source-resolution luminance of the video path: over the footprint rectangle (y0, x0, h, w) of a uint8 source frame
+// [Hs][Ws][3], the centred L [h][w] (rgb8_to_lab_kernel's plane 0: rgb8_lab_f, the same float64 operations) and, when guide !=
+// nullptr, the WLS guide [h][w] (l_to_guide8's).
+__global__ void __launch_bounds__(256) rgb8_to_l_guide_kernel(const unsigned char* __restrict__ rgb, int Ws, int y0, int x0, int h, int w,
+                                                              float* __restrict__ l, unsigned char* __restrict__ guide) {
+  const size_t n = (size_t)h * w;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int y = (int)(i / w), x = (int)(i - (size_t)y * w);
+    double f[3];
+    rgb8_lab_f(rgb + ((size_t)(y0 + y) * Ws + x0 + x) * 3, f);
+    const float v = (float)(116.0 * f[1] - 16.0) - 50.0f;
+    l[i] = v;
+    if (guide) guide[i] = guide8_of_l(v);
+  }
+}
+
+// The window's ab [planes][Ho][Wo] resampled onto the footprint (fy, fx, h, w) of the source grid: source pixel (ys, xs) sits at
+// window coordinate cy = ((2 ys + 1) Hr - (2 oy + 1) Hs) / (2 Hs) (an exact integer numerator, one float64 division; cx the
+// same), clamped to the window, and takes upsample2_kernel's bilinear expression with every operation separately rounded.
+__global__ void __launch_bounds__(256) ab_to_source_kernel(const float* __restrict__ ab, int planes, int Ho, int Wo, int Hs, int Ws, int Hr,
+                                                           int Wr, int oy, int ox, int fy, int fx, int h, int w, float* __restrict__ dst) {
+  const size_t n = (size_t)planes * h * w;
+  for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n; idx += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(idx % w);
+    const size_t t = idx / w;
+    const int y = (int)(t % h);
+    const size_t pl = t / h;
+    const long long ny = (2LL * (fy + y) + 1) * Hr - (2LL * oy + 1) * Hs, nx = (2LL * (fx + x) + 1) * Wr - (2LL * ox + 1) * Ws;
+    const double cy = fmin(fmax(__ddiv_rn((double)ny, 2.0 * Hs), 0.0), (double)(Ho - 1));
+    const double cx = fmin(fmax(__ddiv_rn((double)nx, 2.0 * Ws), 0.0), (double)(Wo - 1));
+    const int y0 = (int)floor(cy), x0 = (int)floor(cx);
+    const int y1 = min(y0 + 1, Ho - 1), x1 = min(x0 + 1, Wo - 1);
+    const float ly = (float)(cy - y0), lx = (float)(cx - x0);
+    const float* sp = ab + pl * Ho * Wo;
+    const float v00 = __ldg(sp + (size_t)y0 * Wo + x0), v01 = __ldg(sp + (size_t)y0 * Wo + x1);
+    const float v10 = __ldg(sp + (size_t)y1 * Wo + x0), v11 = __ldg(sp + (size_t)y1 * Wo + x1);
+    const float wy = __fsub_rn(1.f, ly), wx = __fsub_rn(1.f, lx);
+    const float top = __fadd_rn(__fmul_rn(wx, v00), __fmul_rn(lx, v01)), bot = __fadd_rn(__fmul_rn(wx, v10), __fmul_rn(lx, v11));
+    dst[idx] = __fadd_rn(__fmul_rn(wy, top), __fmul_rn(ly, bot));
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ CenterPad resize
 __device__ __forceinline__ int mirror_idx(int i, int n) {  // scipy.ndimage mode="mirror": d c b | a b c d | c b a
   if (n == 1) return 0;
@@ -354,6 +396,15 @@ void launch_l_to_guide8(const float* l, unsigned char* g, size_t n, cudaStream_t
 }
 void launch_rgb8_to_l_half(const unsigned char* rgb, float* l, float* l_half, unsigned char* guide, int H, int W, cudaStream_t s) {
   rgb8_to_l_half_kernel<<<grid_for((size_t)(H / 2) * ((W + 15) / 16) * 32, 256), 256, 0, s>>>(rgb, l, l_half, guide, H, W);
+  launch_counter_add(1);
+}
+void launch_rgb8_to_l_guide(const unsigned char* rgb, int Ws, int y0, int x0, int h, int w, float* l, unsigned char* guide, cudaStream_t s) {
+  rgb8_to_l_guide_kernel<<<grid_for((size_t)h * w, 256), 256, 0, s>>>(rgb, Ws, y0, x0, h, w, l, guide);
+  launch_counter_add(1);
+}
+void launch_ab_to_source(const float* ab, int planes, int Ho, int Wo, const int g[6], const int fp[4], float* dst, cudaStream_t s) {
+  ab_to_source_kernel<<<grid_for((size_t)planes * fp[2] * fp[3], 256), 256, 0, s>>>(ab, planes, Ho, Wo, g[0], g[1], g[2], g[3], g[4], g[5],
+                                                                                    fp[0], fp[1], fp[2], fp[3], dst);
   launch_counter_add(1);
 }
 void launch_gauss_axis_u8(const unsigned char* src, double* dst, const double* w, int radius, size_t n_outer, int len, int inner,

@@ -31,7 +31,7 @@ EXPORTED = [
     "dvc_corr_set_peer_outputs", "dvc_set_exemplars", "dvc_colorize_frames_exemplars", "dvc_colorize_clip_exemplars",
     "dvc_corr_softmax_warp_exemplars", "dvc_colorize_video_rgb8", "dvc_colorize_frames_clips", "dvc_colorize_clips",
     "dvc_colorize_videos_rgb8", "dvc_colorize_frames_clips_exemplars", "dvc_colorize_clips_exemplars",
-    "dvc_colorize_videos_exemplars_rgb8",
+    "dvc_colorize_videos_exemplars_rgb8", "dvc_source_footprint", "dvc_ab_to_source", "dvc_colorize_videos_source_rgb8",
 ]
 
 _lib = None
@@ -92,6 +92,10 @@ def load_library():
                                                      c_void]
         lib.dvc_colorize_videos_exemplars_rgb8.argtypes = [c_void, c_int, P(c_int), P(c_void), c_int, P(c_int), c_int, c_int, c_float,
                                                            c_void, c_int, c_float, c_float, c_void, c_void, c_void]
+        lib.dvc_source_footprint.argtypes = [c_int] * 8 + [P(c_int)]
+        lib.dvc_ab_to_source.argtypes = [c_void, c_void] + [c_int] * 9 + [c_void, c_void]
+        lib.dvc_colorize_videos_source_rgb8.argtypes = [c_void, c_int, P(c_int), P(c_void), c_int, P(c_int), c_int, c_int, c_float,
+                                                        c_void, c_int, c_float, c_float, P(c_void), c_void, c_void]
         lib.dvc_exemplar_pack_size.argtypes = [c_void, c_int, c_int]
         lib.dvc_exemplar_pack_size.restype = c_i64
         lib.dvc_exemplar_export.argtypes = [c_void, c_void, c_i64, c_void]
@@ -603,6 +607,77 @@ class Context:
         self._check(rc, "dvc_colorize_videos_exemplars_rgb8")
         return (out, last) if return_last else out
 
+    # ---- output at the source resolution: the window's chroma on each source frame's own luminance -------------------------
+    def ab_to_source(self, ab, geometry, size):
+        """The window ab [...,Ho,Wo] (CUDA float32, size = (Ho, Wo)) resampled bilinearly onto the source footprint of
+        geometry = (Hs, Ws, Hr, Wr, oy, ox): [...,h,w] (include/dvc.h: dvc_ab_to_source)."""
+        ab = _dev_f32(ab, "ab_to_source input")
+        Ho, Wo = int(size[0]), int(size[1])
+        if ab.dim() < 2 or tuple(ab.shape[-2:]) != (Ho, Wo):
+            raise DvcError("ab_to_source: the planes must be [...,Ho,Wo] with (Ho, Wo) = size")
+        g = [int(v) for v in geometry]
+        _, _, h, w = source_footprint(*g, Ho, Wo)
+        out = torch.empty(*ab.shape[:-2], h, w, device=ab.device, dtype=torch.float32)
+        planes = ab.numel() // (Ho * Wo)
+        self._check(self.lib.dvc_ab_to_source(self.h, _ptr(ab), planes, Ho, Wo, *g, _ptr(out), _stream(ab.device)), "dvc_ab_to_source")
+        return out
+
+    def colorize_videos_source_rgb8(self, clips, K, size, temperature=1e-10, first_last_lab=None, wls=(500.0, 4.0), out=None,
+                                    return_last=False):
+        """colorize_videos_exemplars_rgb8 with every frame at its source resolution: a list of S uint8 tensors
+        [K[s],F,h_s,w_s,3], (h_s, w_s) the footprint of clip s's window (source_footprint), drawn with the source frame's own
+        luminance and the network's chroma.  The networks still run at `size`; first_last_lab and the returned last state are
+        [R,3,size[0]/2,size[1]/2] as there.  `out`: None or a list of S such tensors on the side where the clips live."""
+        from dvc.prepost import centerpad_geometry
+
+        what = "colorize_videos_source_rgb8"
+        clips = list(clips)
+        if not clips or not all(isinstance(f, torch.Tensor) and f.dtype == torch.uint8 and f.dim() == 4 and f.shape[3] == 3
+                                for f in clips):
+            raise DvcError(f"{what}: expected a list of uint8 tensors [F,Hs,Ws,3]")
+        on_device = clips[0].is_cuda
+        if any(f.is_cuda != on_device for f in clips) or len({f.shape[0] for f in clips}) != 1:
+            raise DvcError(f"{what}: the clips must have the same frame count and all live on the host or all on the device")
+        clips = [f.contiguous() for f in clips]
+        if not on_device:
+            clips = [f if f.is_pinned() else f.pin_memory() for f in clips]
+        S, F_ = len(clips), clips[0].shape[0]
+        K, ck = self._counts(K, S, what)
+        R = sum(K)
+        Ho, Wo = int(size[0]), int(size[1])
+        geom, shapes = [], []
+        for f, k in zip(clips, K):
+            g = [f.shape[1], f.shape[2], *centerpad_geometry(f.shape[1], f.shape[2], (Ho, Wo))]
+            _, _, h, w = source_footprint(*g, Ho, Wo)
+            geom += g
+            shapes.append((k, F_, h, w, 3))
+
+        def host_or_device(shape, dtype):
+            t = torch.empty(*shape, dtype=dtype, device=clips[0].device)
+            return t if on_device else t.pin_memory()
+
+        if out is None:
+            out = [host_or_device(shp, torch.uint8) for shp in shapes]
+        out = list(out)
+        if len(out) != S or any(o.is_cuda != on_device or o.dtype != torch.uint8 or not o.is_contiguous() or tuple(o.shape) != shp
+                                for o, shp in zip(out, shapes)):
+            raise DvcError(f"{what}: `out` must be a list of contiguous uint8 [K[s],F,h_s,w_s,3] tensors (the footprints) on the "
+                           "same side as the clips")
+        fl = None
+        if first_last_lab is not None:
+            fl = first_last_lab.to(torch.float32).contiguous()
+            if tuple(fl.shape) != (R, 3, Ho // 2, Wo // 2):
+                raise DvcError(f"{what}: first_last_lab must be [R,3,H/2,W/2]")
+        last = host_or_device((R, 3, Ho // 2, Wo // 2), torch.float32) if return_last else None
+        lam, sigma = (0.0, 1.0) if wls is None else (float(wls[0]), float(wls[1]))
+        ptrs = (ctypes.c_void_p * S)(*[f.data_ptr() for f in clips])
+        optrs = (ctypes.c_void_p * S)(*[o.data_ptr() for o in out])
+        g = (ctypes.c_int * (6 * S))(*geom)
+        rc = self.lib.dvc_colorize_videos_source_rgb8(self.h, S, ck, ptrs, F_, g, Ho, Wo, float(temperature), _ptr(fl),
+                                                      0 if wls is None else 1, lam, sigma, optrs, _ptr(last), _stream(self.device))
+        self._check(rc, f"dvc_{what}")
+        return (out, last) if return_last else out
+
     # ---- pre / post-processing around the nets (test.py:58,71,100-102) ----------------------------------
     def resize_half(self, x):
         """F.interpolate(x, scale_factor=0.5, mode="bilinear") for a CUDA [B,C,H,W] tensor with even H, W."""
@@ -826,6 +901,17 @@ def _raw_view(ptr, n_floats, device):
     h = _Holder()
     h.__cuda_array_interface__ = {"shape": (n_floats,), "typestr": "<f4", "data": (ptr, False), "version": 2}
     return torch.as_tensor(h, device=device)
+
+
+def source_footprint(Hs, Ws, Hr, Wr, oy, ox, Ho, Wo):
+    """(y0, x0, h, w): the source pixels of geometry (Hs, Ws, Hr, Wr, oy, ox) whose centres fall inside the (Ho, Wo) window's
+    extent, the size of colorize_videos_source_rgb8's output frames (include/dvc.h: dvc_source_footprint).  Needs no GPU."""
+    fp = (ctypes.c_int * 4)()
+    rc = load_library().dvc_source_footprint(int(Hs), int(Ws), int(Hr), int(Wr), int(oy), int(ox), int(Ho), int(Wo), fp)
+    if rc != 0:
+        raise DvcError(f"dvc_source_footprint failed ({rc}): geometry {(Hs, Ws, Hr, Wr, oy, ox)} has no source pixel inside the "
+                       f"{Ho}x{Wo} window, or a size < 1")
+    return tuple(fp)
 
 
 _contexts = {}

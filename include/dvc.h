@@ -241,6 +241,37 @@ int dvc_colorize_videos_exemplars_rgb8(dvc_ctx* ctx, int S, const int* K, const 
                                        int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda,
                                        float wls_sigma, unsigned char* out, float* last_lab_out, void* stream);
 
+/* ---- video output at the source resolution ---------------------------------------------------------------------------------
+ * The networks run at the CenterPad window (Ho, Wo) = image_size; the reference leaves rescaling the output to the user.
+ * These calls keep the source frame's own luminance and take only the chroma from the network: the window's ab (after x2 * 1.25)
+ * is resampled bilinearly onto the source grid, WLS-filtered with the guide of the source frame's L and turned into sRGB with
+ * that L -- test.py:100-119's recipe, run one grid further.  The output covers the footprint: the source pixels whose centres
+ * fall inside the window's extent [-0.5, Ho - 0.5] x [-0.5, Wo - 0.5], i.e. the whole frame when the source has the window's
+ * aspect ratio or the window zero-pads it, the centre band when CenterPad crops. */
+
+/* Footprint of the window (Ho, Wo) on a source of geometry (Hs, Ws, Hr, Wr, oy, ox) (dvc_colorize_video_rgb8's): source row ys
+ * is in it iff 2 oy Hs <= (2 ys + 1) Hr <= 2 (oy + Ho) Hs (exact integers; columns alike).  out[4] = (y0, x0, h, w).  Needs no
+ * context or device.  DVC_ERR_ARG for a null out or a size < 1, DVC_ERR_SHAPE when no source pixel centre is inside. */
+int dvc_source_footprint(int Hs, int Ws, int Hr, int Wr, int oy, int ox, int Ho, int Wo, int out[4]);
+/* dev_ab [planes,Ho,Wo] (window grid) -> dev_dst [planes,h,w] on the footprint (y0, x0, h, w) of the source grid: pixel (ys, xs)
+ * samples the window at cy = ((2 ys + 1) Hr - (2 oy + 1) Hs) / (2 Hs) (an exact integer numerator over one float64 division; cx
+ * alike) clamped to [0, Ho - 1], bilinearly with dvc_upsample2_scaled's expression, every fp32 operation separately rounded.
+ * With Hs = Hr = Ho and oy = 0 (ditto x) it is the identity. */
+int dvc_ab_to_source(dvc_ctx* ctx, const float* dev_ab, int planes, int Ho, int Wo, int Hs, int Ws, int Hr, int Wr, int oy, int ox,
+                     float* dev_dst, void* stream);
+/* dvc_colorize_videos_exemplars_rgb8 (S clips, K[s] exemplars each; S = 1, K = (1) is the single-clip case) with every output
+ * frame at its source resolution: out[s] points to clip s's own [K[s],F,h_s,w_s,3] uint8, (h_s, w_s) its footprint.  Per row:
+ * the window ab -> dvc_ab_to_source -> if wls, the FGS of its a / b planes (wls_lambda, wls_sigma) guided by dvc_l_to_guide8 of the
+ * source L -> dvc_lab_to_rgb8 with the source L, where the source L is dvc_rgb8_to_lab's plane 0 of the source frame over the
+ * footprint.  lambda and sigma keep their per-pixel meaning: a 1080x1920 grid is 2.5x finer per axis than 432x768, so the
+ * same lambda smooths over a 2.5x smaller fraction of the frame, and the caller may raise it.  The networks, the
+ * recurrence, first_last_lab and last_lab_out are those of the window-size call ([R,3,Ho/2,Wo/2]), so chunked calls continue a
+ * clip exactly.  Refuses what that call refuses, plus a null out or out[s], before any launch.  Device memory does not depend
+ * on F.  Synchronises `stream` before returning. */
+int dvc_colorize_videos_source_rgb8(dvc_ctx* ctx, int S, const int* K, const unsigned char* const* frames, int F, const int* geom,
+                                    int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda,
+                                    float wls_sigma, unsigned char* const* out, float* last_lab_out, void* stream);
+
 /* ---- pre / post-processing around the nets (SURVEY.md §8f row 1) ------------------------------ */
 
 /* F.interpolate(x, scale_factor=0.5, mode="bilinear") -- test.py:58,71.  dev_src [planes,H,W] (H, W even) ->

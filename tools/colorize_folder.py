@@ -26,6 +26,11 @@ that has frames left: n = min(--chunk, the run of frames of one source size each
 out, it leaves with its rows: the others continue with dvc_set_exemplars of their exemplars and their rows of the previous
 call's last_lab_out.
 
+--source-resolution writes every frame at its source resolution instead of --image-size: the networks still run at
+--image-size, and every call is dvc_colorize_videos_source_rgb8 (same chunks, exemplars and recurrence), which resamples the
+network's colour onto the source frame, WLS-filters it against the source frame's own luminance and keeps that luminance.
+The PNGs cover the part of the frame the window covers (dvc_source_footprint): the whole frame unless CenterPad crops it.
+
 What the reference does and this script does not: the AVI writer (folder2vid).  Image decode / encode stays on the host
 (PIL), as in the reference.  Without checkpoints (none ship with the reference tree) pass --seeded-weights to run the
 pipeline on the seeded random weights of dvc/synth.py (useful as a smoke run only).
@@ -109,6 +114,9 @@ def main():
     ap.add_argument("--fast", action="store_true",
                     help="one MMA per convolution product (dvc.MATH_FP16X1: 11-bit conv operands, the precision of the "
                          "reference's cuDNN convolutions on a GPU) instead of the fp32-class default")
+    ap.add_argument("--source-resolution", action="store_true",
+                    help="write every frame at its source resolution (the part of the frame the --image-size window covers): the "
+                         "network's colour resampled onto the source frame and WLS-filtered against its own luminance")
     args = ap.parse_args()
     if args.chunk < 1:
         raise SystemExit("--chunk must be >= 1")
@@ -129,6 +137,7 @@ def main():
         raise SystemExit(f"--ref: at most 8 exemplars in one pass, got {sum(counts)}")
 
     import dvc
+    from dvc.prepost import centerpad_geometry
     from dvc.synth import make_state_dict
 
     ctx = dvc.get_context(0)
@@ -207,19 +216,36 @@ def main():
         for f in writes[slot]:  # the encodes of chunk i-2 still read this output slot
             f.result()
         rows = sum(counts[s] for s in active)
-        if ring_out[slot] is None or tuple(ring_out[slot].shape[:2]) != (rows, n):
-            ring_out[slot] = torch.empty(rows, n, H, W, 3, dtype=torch.uint8).pin_memory()
-        if S == 1:
+        if args.source_resolution:  # every clip's frames at its footprint, one [K_s,n,h,w,3] buffer per clip
+            shapes = []
+            for chunk in chunks:
+                Hs, Ws = chunk[0][1].shape[:2]
+                _, _, h, w = dvc.source_footprint(Hs, Ws, *centerpad_geometry(Hs, Ws, (H, W)), H, W)
+                shapes.append((h, w))
+            shapes = [(counts[s], n, h, w, 3) for s, (h, w) in zip(active, shapes)]
+            if ring_out[slot] is None or [tuple(o.shape) for o in ring_out[slot]] != shapes:
+                ring_out[slot] = [torch.empty(shp, dtype=torch.uint8).pin_memory() for shp in shapes]
+            res, last = ctx.colorize_videos_source_rgb8([ring_in[slot][s][:n] for s in active], [counts[s] for s in active], (H, W),
+                                                        args.temperature, first_last_lab=last, wls=wls, out=ring_out[slot],
+                                                        return_last=True)
+            arr = [row for o in res for row in o.numpy()]
+            dests = [(d, chunk) for s, chunk in zip(active, chunks) for d in outs[s]]
+        elif S == 1:
+            if ring_out[slot] is None or tuple(ring_out[slot].shape[:2]) != (rows, n):
+                ring_out[slot] = torch.empty(rows, n, H, W, 3, dtype=torch.uint8).pin_memory()
             out, last = ctx.colorize_video_rgb8(ring_in[slot][0][:n], (H, W), args.temperature, first_last_lab=last, wls=wls,
                                                 out=ring_out[slot], return_last=True)
             dests = [(d, chunks[0]) for d in outs[0]]
+            arr = out.numpy()
         else:
+            if ring_out[slot] is None or tuple(ring_out[slot].shape[:2]) != (rows, n):
+                ring_out[slot] = torch.empty(rows, n, H, W, 3, dtype=torch.uint8).pin_memory()
             out, last = ctx.colorize_videos_exemplars_rgb8([ring_in[slot][s][:n] for s in active], [counts[s] for s in active], (H, W),
                                                            args.temperature, first_last_lab=last, wls=wls, out=ring_out[slot],
                                                            return_last=True)
             dests = [(d, chunk) for s, chunk in zip(active, chunks) for d in outs[s]]
-        arr = out.numpy()
-        writes[slot] = [encode.submit(save_png, arr[r, t], os.path.join(d, os.path.splitext(name)[0] + ".png"))
+            arr = out.numpy()
+        writes[slot] = [encode.submit(save_png, arr[r][t],os.path.join(d, os.path.splitext(name)[0] + ".png"))
                         for r, (d, chunk) in enumerate(dests) for t, (name, _) in enumerate(chunk)]
         for s in active:
             done[s] += n
