@@ -1937,6 +1937,22 @@ struct VideoIO {
   float* last_out = nullptr;     // [R][3][Ho/2][Wo/2] or nullptr
   std::vector<double> taps;      // every source's [wy | wx | 1.0]: uploaded once per call
   float lut[256];
+  // JPEG output instead of sRGB (dvc_colorize_videos_jpeg): one encoder per output size (the window, or each footprint group)
+  // over the rows of the rgb slot; frame t of row r goes to out[clip] + (r_local F + t) stride and sizes[r F + t]
+  struct Jpeg {
+    int B = 0, H = 0, W = 0;
+    size_t rgb0 = 0;  // its first row in the rgb slot
+    JpegLayout L;
+    JpegQuant q;
+    unsigned char header[kJpegHeaderBytes];
+    std::vector<unsigned char*> dst;  // per row: device-visible base of its [F] slots
+    std::vector<int64_t*> size;       // per row: device-visible sizes + r F
+    unsigned char* ws = nullptr;
+    void** tabs = nullptr;            // device copy of dst | size
+  };
+  bool jpeg = false;
+  int64_t jpeg_stride = 0;
+  std::vector<Jpeg> enc;
   // source-resolution output instead of `out`: the clips grouped by footprint size, pixels of one frame of every footprint, of
   // every row's footprint, and the largest of one group (the FGS scratch is reused group after group)
   bool source = false;
@@ -2005,6 +2021,16 @@ static int video_prologue(dvc_ctx* c, VideoIO& v, int R, cudaStream_t s) {
     }
   }
   CUDA_TRY(c, cudaMemcpyAsync(v.dtaps, v.taps.data(), v.taps.size() * 8, cudaMemcpyHostToDevice, s));
+  for (size_t i = 0; i < v.enc.size(); ++i) {  // the encoders run one after another on stream P: one workspace each
+    VideoIO::Jpeg& e = v.enc[i];
+    const std::string n = "jpeg" + std::to_string(i);
+    DVC_TRY(raw((n + ".ws").c_str(), e.L.bytes, &e.ws));
+    DVC_TRY(raw((n + ".tabs").c_str(), 2 * e.B * sizeof(void*), &e.tabs));
+    std::vector<void*> tabs(e.dst.begin(), e.dst.end());
+    tabs.insert(tabs.end(), e.size.begin(), e.size.end());
+    CUDA_TRY(c, cudaMemcpyAsync(e.ws + e.L.header, e.header, kJpegHeaderBytes, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(c, cudaMemcpyAsync(e.tabs, tabs.data(), tabs.size() * sizeof(void*), cudaMemcpyHostToDevice, s));
+  }
   return DVC_OK;
 }
 
@@ -2097,10 +2123,19 @@ static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int
     }
     launch_lab_to_rgb8(Lfull, src, v.abL, rgb, R, v.Ho, v.Wo, inv, c->sP);  // test.py:116-119
   }
+  if (v.jpeg) {  // test.py:120 writes JPEG files: encoded here, each file stored into its slot by the encoder's last launch
+    const unsigned char* slot = v.source ? v.srgb + (size_t)(t & 1) * v.fp_rows * 3 : rgb;
+    for (const VideoIO::Jpeg& e : v.enc) {
+      const JpegDst dst{(unsigned char* const*)e.tabs, (int64_t* const*)(e.tabs + e.B), (int64_t)t * v.jpeg_stride, t};
+      launch_jpeg_encode(slot + e.rgb0, e.B, e.H, e.W, e.q, e.ws, e.L, dst, c->sP);
+    }
+  }
   DVC_TRY(check_launch(c, "video post-processing"));
   CUDA_TRY(c, cudaEventRecord(c->evP[t & 3], c->sP));
   CUDA_TRY(c, cudaStreamWaitEvent(c->sD, c->evP[t & 3], 0));
-  if (v.source) {
+  if (v.jpeg) {
+    // nothing to download: the files are in place when evP[t & 3] fires
+  } else if (v.source) {
     const unsigned char* srgb = v.srgb + (size_t)(t & 1) * v.fp_rows * 3;
     for (const VideoSrc& k : v.clips) {
       const size_t n3 = (size_t)k.fp[2] * k.fp[3] * 3;
@@ -2378,10 +2413,19 @@ extern "C" int dvc_colorize_video_rgb8(dvc_ctx* c, const unsigned char* frames, 
 
 // S clips, clip s with K[s] exemplar rows (K == nullptr: one each), every clip with its own geometry.  The output is `out` at
 // the window size, or clip s's own source_out[s] at its footprint size (source_out != nullptr; K given then).
+struct JpegOut {  // dvc_colorize_videos_jpeg's destination
+  int quality;
+  unsigned char* const* out;
+  int64_t stride;
+  int64_t* sizes;
+};
+static int video_jpeg_outputs(dvc_ctx* c, const char* what, VideoIO& v, const int* K, int F, const JpegOut& j);
+
 static int videos_impl(dvc_ctx* c, const char* what, int S, const int* K, const unsigned char* const* frames, int F, const int* geom,
                        int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
-                       unsigned char* out, float* last_lab_out, void* stream, unsigned char* const* source_out = nullptr) {
-  if (!c || !frames || !geom || (!out && !source_out) || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
+                       unsigned char* out, float* last_lab_out, void* stream, unsigned char* const* source_out = nullptr,
+                       const JpegOut* jpeg = nullptr) {
+  if (!c || !frames || !geom || (!out && !source_out && !jpeg) || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
   const int* counts = K;
   if (K) {
     DVC_TRY(check_counts(c, what, S, K));
@@ -2397,6 +2441,7 @@ static int videos_impl(dvc_ctx* c, const char* what, int S, const int* K, const 
   }
   DVC_TRY(video_finish(c, what, v, wls, wls_lambda, wls_sigma, out, last_lab_out));
   if (source_out) DVC_TRY(video_source_outputs(c, what, v, counts, source_out));
+  if (jpeg) DVC_TRY(video_jpeg_outputs(c, what, v, counts, F, *jpeg));
   return colorize_clip_impl(c, what, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, S, K, nullptr, stream, &v);
 }
 
@@ -2424,6 +2469,125 @@ extern "C" int dvc_colorize_videos_source_rgb8(dvc_ctx* c, int S, const int* K, 
   if (c && !out) return fail(c, DVC_ERR_ARG, std::string(what) + ": out is null");
   return videos_impl(c, what, S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda, wls_sigma, nullptr,
                      last_lab_out, stream, out);
+}
+
+// ---- JPEG output (jpeg.cu) ---------------------------------------------------------------------------------------------
+extern "C" int64_t dvc_jpeg_max_bytes(int H, int W) {
+  const int64_t n = jpeg_max_bytes(H, W);
+  return n < 0 ? DVC_ERR_SHAPE : n;
+}
+
+// A pointer the encoder's kernels store into: device memory as it is, page-locked host memory through its device mapping.
+// Pageable host memory is refused: the kernels cannot reach it.
+static int device_visible(dvc_ctx* c, const char* what, const std::string& name, void* p, void** dp) {
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(c, DVC_ERR_ARG, std::string(what) + ": " + name + " is not a CUDA-visible pointer");
+  }
+  if (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) {
+    *dp = p;
+    return DVC_OK;
+  }
+  if (a.type == cudaMemoryTypeHost && a.devicePointer) {
+    *dp = a.devicePointer;
+    return DVC_OK;
+  }
+  return fail(c, DVC_ERR_ARG, std::string(what) + ": " + name + " is pageable host memory (device or page-locked host memory is needed)");
+}
+
+// The checks of the JPEG destination (before any launch) and one encoder per output size: the window's, over all R rows, or
+// each footprint group's, over the rows of its clips in the order of the source-resolution rgb slot
+static int video_jpeg_outputs(dvc_ctx* c, const char* what, VideoIO& v, const int* K, int F, const JpegOut& j) {
+  if (j.quality < 1 || j.quality > 100) return fail(c, DVC_ERR_ARG, std::string(what) + ": quality must be in [1, 100]");
+  if (!j.out || !j.sizes) return fail(c, DVC_ERR_ARG, std::string(what) + ": out / sizes is null");
+  const size_t S = v.clips.size();
+  std::vector<unsigned char*> out(S);
+  std::vector<int> row0(S);
+  int R = 0;
+  for (size_t s = 0; s < S; ++s) {
+    if (!j.out[s]) return fail(c, DVC_ERR_ARG, std::string(what) + ": out[" + std::to_string(s) + "] is null");
+    void* d = nullptr;
+    DVC_TRY(device_visible(c, what, "out[" + std::to_string(s) + "]", j.out[s], &d));
+    out[s] = (unsigned char*)d, row0[s] = R, R += K[s];
+  }
+  void* sizes = nullptr;
+  DVC_TRY(device_visible(c, what, "sizes", j.sizes, &sizes));
+  int tables[2][64];
+  const JpegQuant q = jpeg_quant(j.quality, tables);
+  auto add = [&](int H, int W, size_t rgb0, const std::vector<int>& clips) {
+    const int64_t need = jpeg_max_bytes(H, W);
+    if (need < 0 || j.stride < need)
+      return fail(c, DVC_ERR_SHAPE, std::string(what) + ": stride " + std::to_string(j.stride) + " is below dvc_jpeg_max_bytes(" +
+                                        std::to_string(H) + ", " + std::to_string(W) + ") = " + std::to_string(need));
+    VideoIO::Jpeg e;
+    e.H = H, e.W = W, e.rgb0 = rgb0, e.q = q;
+    jpeg_header(H, W, tables, e.header);
+    for (int s : clips)
+      for (int r = 0; r < K[s]; ++r) {
+        e.dst.push_back(out[s] + (size_t)r * F * j.stride);
+        e.size.push_back((int64_t*)sizes + (size_t)(row0[s] + r) * F);
+      }
+    e.B = (int)e.dst.size();
+    e.L = jpeg_layout(e.B, H, W);
+    v.enc.push_back(std::move(e));
+    return (int)DVC_OK;
+  };
+  if (v.source) {
+    for (const auto& g : v.groups) {
+      const VideoSrc& k0 = v.clips[g[0]];
+      DVC_TRY(add(k0.fp[2], k0.fp[3], k0.srgb0, g));
+    }
+  } else {
+    std::vector<int> all(S);
+    for (size_t s = 0; s < S; ++s) all[s] = (int)s;
+    DVC_TRY(add(v.Ho, v.Wo, 0, all));
+  }
+  v.jpeg = true, v.jpeg_stride = j.stride;
+  return DVC_OK;
+}
+
+extern "C" int dvc_colorize_videos_jpeg(dvc_ctx* c, int S, const int* K, const unsigned char* const* frames, int F, const int* geom,
+                                        int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda,
+                                        float wls_sigma, int source_resolution, int quality, unsigned char* const* out, int64_t stride,
+                                        int64_t* sizes, float* last_lab_out, void* stream) {
+  const char* what = "colorize_videos_jpeg";
+  if (c && !K) return fail(c, DVC_ERR_ARG, std::string(what) + ": K is null");
+  if (c && (!out || !sizes)) return fail(c, DVC_ERR_ARG, std::string(what) + ": out / sizes is null");
+  const JpegOut j{quality, out, stride, sizes};
+  return videos_impl(c, what, S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda, wls_sigma, nullptr,
+                     last_lab_out, stream, source_resolution ? out : nullptr, &j);
+}
+
+extern "C" int dvc_encode_jpeg(dvc_ctx* c, const unsigned char* dev_rgb, int B, int H, int W, int quality, unsigned char* out,
+                               int64_t stride, int64_t* sizes, void* stream) {
+  const char* what = "encode_jpeg";
+  if (!c || !dev_rgb || !out || !sizes || B < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
+  if (quality < 1 || quality > 100) return fail(c, DVC_ERR_ARG, std::string(what) + ": quality must be in [1, 100]");
+  const int64_t need = jpeg_max_bytes(H, W);
+  if (need < 0) return fail(c, DVC_ERR_SHAPE, std::string(what) + ": H, W must be in [1, 65535] (and the frame below ~14 Mpixel)");
+  if (stride < need)
+    return fail(c, DVC_ERR_SHAPE, std::string(what) + ": stride " + std::to_string(stride) + " is below dvc_jpeg_max_bytes = " + std::to_string(need));
+  CUDA_TRY(c, cudaSetDevice(c->device));
+  void *dout = nullptr, *dsizes = nullptr;
+  DVC_TRY(device_visible(c, what, "out", out, &dout));
+  DVC_TRY(device_visible(c, what, "sizes", sizes, &dsizes));
+  cudaStream_t s = (cudaStream_t)stream;
+  const JpegLayout L = jpeg_layout(B, H, W);
+  void *ws = nullptr, *tabs = nullptr;
+  DVC_TRY(get_raw(c, "jpeg.ws", L.bytes, &ws, s));
+  DVC_TRY(get_raw(c, "jpeg.tabs", 2 * (size_t)B * sizeof(void*), &tabs, s));
+  int tables[2][64];
+  const JpegQuant q = jpeg_quant(quality, tables);
+  unsigned char header[kJpegHeaderBytes];
+  jpeg_header(H, W, tables, header);
+  std::vector<void*> tab(2 * (size_t)B);
+  for (int b = 0; b < B; ++b) tab[b] = (unsigned char*)dout + (size_t)b * stride, tab[B + b] = (int64_t*)dsizes + b;
+  CUDA_TRY(c, cudaMemcpyAsync((unsigned char*)ws + L.header, header, kJpegHeaderBytes, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(c, cudaMemcpyAsync(tabs, tab.data(), tab.size() * sizeof(void*), cudaMemcpyHostToDevice, s));
+  const JpegDst dst{(unsigned char* const*)tabs, (int64_t* const*)tabs + B, 0, 0};
+  launch_jpeg_encode(dev_rgb, B, H, W, q, (unsigned char*)ws, L, dst, s);
+  return check_launch(c, what);
 }
 
 extern "C" int dvc_ab_to_source(dvc_ctx* c, const float* dev_ab, int planes, int Ho, int Wo, int Hs, int Ws, int Hr, int Wr, int oy, int ox,

@@ -311,6 +311,37 @@ void launch_gauss_axis_f64(const double* src, double* dst, const double* w, int 
 void launch_zoom_crop(const double* src, int Hs, int Ws, int Hr, int Wr, int oy, int ox, unsigned char* dst, int Ho, int Wo,
                       cudaStream_t s);
 
+// Baseline JPEG encoder (jpeg.cu).  Header bytes (SOI .. SOS, identical for every size and quality) and the worst-case bits of
+// one 8x8 block: DC code <= 11 + value 11 bits, 63 AC coefficients of <= 16 + 10 bits (include/dvc.h: dvc_jpeg_max_bytes).
+constexpr int kJpegHeaderBytes = 623;
+constexpr int64_t kJpegMaxBlockBits = 22 + 63 * 26;
+struct JpegQuant {  // per table (luma, chroma) and natural index: jcdctmgr.c's reciprocal, correction and total shift
+  uint16_t recip[2][64];
+  uint16_t corr[2][64];
+  uint8_t shift[2][64];
+};
+// image b's file goes to dst[b] + dst_off, its size to size[b][size_off] (device-visible pointers)
+struct JpegDst {
+  unsigned char* const* dst;
+  int64_t* const* size;
+  int64_t dst_off;
+  int64_t size_off;
+};
+// byte offsets of the encoder's workspaces for a batch of B images of H x W
+struct JpegLayout {
+  int64_t nblk = 0;
+  int ntile = 0;
+  size_t words_per_image = 0, file_stride = 0;
+  size_t coef = 0, acbits = 0, off = 0, words = 0, cnt = 0, ffoff = 0, totals = 0, header = 0, file = 0, bytes = 0;
+};
+int64_t jpeg_max_bytes(int H, int W);  // -1 outside H, W in [1, 65535] with fewer than 2^31 worst-case bits
+JpegQuant jpeg_quant(int quality, int tables[2][64]);
+void jpeg_header(int H, int W, const int tables[2][64], unsigned char out[kJpegHeaderBytes]);
+JpegLayout jpeg_layout(int B, int H, int W);
+// B images rgb [B][H][W][3] (device) -> JFIF files; ws (L.bytes, device) holds the header at L.header; 7 launches
+void launch_jpeg_encode(const unsigned char* rgb, int B, int H, int W, const JpegQuant& qt, unsigned char* ws, const JpegLayout& L,
+                        const JpegDst& dst, cudaStream_t s);
+
 int64_t launch_counter_add(int64_t n);  // global launch counter (introspection)
 
 }  // namespace dvc

@@ -32,6 +32,7 @@ EXPORTED = [
     "dvc_corr_softmax_warp_exemplars", "dvc_colorize_video_rgb8", "dvc_colorize_frames_clips", "dvc_colorize_clips",
     "dvc_colorize_videos_rgb8", "dvc_colorize_frames_clips_exemplars", "dvc_colorize_clips_exemplars",
     "dvc_colorize_videos_exemplars_rgb8", "dvc_source_footprint", "dvc_ab_to_source", "dvc_colorize_videos_source_rgb8",
+    "dvc_jpeg_max_bytes", "dvc_encode_jpeg", "dvc_colorize_videos_jpeg",
 ]
 
 _lib = None
@@ -96,6 +97,11 @@ def load_library():
         lib.dvc_ab_to_source.argtypes = [c_void, c_void] + [c_int] * 9 + [c_void, c_void]
         lib.dvc_colorize_videos_source_rgb8.argtypes = [c_void, c_int, P(c_int), P(c_void), c_int, P(c_int), c_int, c_int, c_float,
                                                         c_void, c_int, c_float, c_float, P(c_void), c_void, c_void]
+        lib.dvc_jpeg_max_bytes.argtypes = [c_int, c_int]
+        lib.dvc_jpeg_max_bytes.restype = c_i64
+        lib.dvc_encode_jpeg.argtypes = [c_void, c_void, c_int, c_int, c_int, c_int, c_void, c_i64, c_void, c_void]
+        lib.dvc_colorize_videos_jpeg.argtypes = [c_void, c_int, P(c_int), P(c_void), c_int, P(c_int), c_int, c_int, c_float, c_void,
+                                                 c_int, c_float, c_float, c_int, c_int, P(c_void), c_i64, c_void, c_void, c_void]
         lib.dvc_exemplar_pack_size.argtypes = [c_void, c_int, c_int]
         lib.dvc_exemplar_pack_size.restype = c_i64
         lib.dvc_exemplar_export.argtypes = [c_void, c_void, c_i64, c_void]
@@ -678,6 +684,95 @@ class Context:
         self._check(rc, f"dvc_{what}")
         return (out, last) if return_last else out
 
+    # ---- JPEG output (test.py:120): files byte-identical to Pillow's, only the compressed bytes leave the device ----------------
+    def encode_jpeg_into(self, rgb, out, sizes, quality=75):
+        """Encode the CUDA uint8 images rgb [B,H,W,3] into out [B,stride] uint8 and sizes [B] int64, both CUDA or pinned CPU
+        tensors (include/dvc.h: dvc_encode_jpeg).  Asynchronous on the current stream."""
+        if not (isinstance(rgb, torch.Tensor) and rgb.is_cuda and rgb.dtype == torch.uint8 and rgb.dim() == 4 and rgb.shape[3] == 3):
+            raise DvcError("encode_jpeg: expected a CUDA uint8 tensor [B,H,W,3]")
+        rgb = rgb.contiguous()
+        B, H, W, _ = rgb.shape
+        if (out.dtype != torch.uint8 or out.dim() != 2 or out.shape[0] != B or out.stride(1) != 1 or sizes.dtype != torch.int64
+                or tuple(sizes.shape) != (B,) or not sizes.is_contiguous()):
+            raise DvcError("encode_jpeg: out must be uint8 [B,stride] (rows contiguous) and sizes int64 [B]")
+        rc = self.lib.dvc_encode_jpeg(self.h, _ptr(rgb), B, H, W, int(quality), _ptr(out), out.stride(0), _ptr(sizes),
+                                      _stream(self.device))
+        self._check(rc, "dvc_encode_jpeg")
+
+    def encode_jpeg(self, rgb, quality=75):
+        """The JFIF files of the CUDA uint8 images rgb [B,H,W,3] (or one [H,W,3]) as a list of bytes, equal to
+        PIL.Image.fromarray(x).save(f, "JPEG", quality=quality).  Synchronises the current stream."""
+        if rgb.dim() == 3:
+            rgb = rgb.unsqueeze(0)
+        B, H, W = rgb.shape[0], rgb.shape[1], rgb.shape[2]
+        out = torch.empty(B, jpeg_max_bytes(H, W), dtype=torch.uint8).pin_memory()
+        sizes = torch.empty(B, dtype=torch.int64).pin_memory()
+        self.encode_jpeg_into(rgb, out, sizes, quality)
+        torch.cuda.current_stream(self.device).synchronize()
+        return [out[b, :int(sizes[b])].numpy().tobytes() for b in range(B)]
+
+    def colorize_videos_jpeg(self, clips, K, size, quality=75, source_resolution=False, temperature=1e-10, first_last_lab=None,
+                             wls=(500.0, 4.0), out=None, sizes=None, return_last=False):
+        """colorize_videos_exemplars_rgb8 (window output) or colorize_videos_source_rgb8 (source_resolution=True) with every frame
+        encoded as encode_jpeg encodes it, on the device (include/dvc.h: dvc_colorize_videos_jpeg).  Returns (slots, sizes): slots a
+        list of S uint8 tensors [K[s],F,stride], sizes int64 [R,F]; jpeg_files(slots, sizes) cuts the files out.  stride is
+        jpeg_max_bytes of the largest output frame.  `out` / `sizes`: None or such tensors on the side where the clips live
+        (pinned CPU or CUDA).  first_last_lab and the returned last state as in the rgb8 calls ([R,3,size[0]/2,size[1]/2])."""
+        from dvc.prepost import centerpad_geometry
+
+        what = "colorize_videos_jpeg"
+        clips = list(clips)
+        if not clips or not all(isinstance(f, torch.Tensor) and f.dtype == torch.uint8 and f.dim() == 4 and f.shape[3] == 3
+                                for f in clips):
+            raise DvcError(f"{what}: expected a list of uint8 tensors [F,Hs,Ws,3]")
+        on_device = clips[0].is_cuda
+        if any(f.is_cuda != on_device for f in clips) or len({f.shape[0] for f in clips}) != 1:
+            raise DvcError(f"{what}: the clips must have the same frame count and all live on the host or all on the device")
+        clips = [f.contiguous() for f in clips]
+        if not on_device:
+            clips = [f if f.is_pinned() else f.pin_memory() for f in clips]
+        S, F_ = len(clips), clips[0].shape[0]
+        K, ck = self._counts(K, S, what)
+        R = sum(K)
+        Ho, Wo = int(size[0]), int(size[1])
+        geom, stride = [], jpeg_max_bytes(Ho, Wo)
+        for f in clips:
+            g = [f.shape[1], f.shape[2], *centerpad_geometry(f.shape[1], f.shape[2], (Ho, Wo))]
+            geom += g
+            if source_resolution:
+                _, _, h, w = source_footprint(*g, Ho, Wo)
+                stride = max(stride, jpeg_max_bytes(h, w))
+
+        def host_or_device(shape, dtype):
+            t = torch.empty(*shape, dtype=dtype, device=clips[0].device)
+            return t if on_device else t.pin_memory()
+
+        if out is None:
+            out = [host_or_device((k, F_, stride), torch.uint8) for k in K]
+        out = list(out)
+        if len(out) != S or any(o.dtype != torch.uint8 or not o.is_contiguous() or o.dim() != 3 or tuple(o.shape[:2]) != (k, F_)
+                                for o, k in zip(out, K)) or len({o.shape[2] for o in out}) != 1:
+            raise DvcError(f"{what}: `out` must be a list of contiguous uint8 [K[s],F,stride] tensors with one stride")
+        if sizes is None:
+            sizes = host_or_device((R, F_), torch.int64)
+        if sizes.dtype != torch.int64 or not sizes.is_contiguous() or tuple(sizes.shape) != (R, F_):
+            raise DvcError(f"{what}: sizes must be a contiguous int64 [R,F] tensor")
+        fl = None
+        if first_last_lab is not None:
+            fl = first_last_lab.to(torch.float32).contiguous()
+            if tuple(fl.shape) != (R, 3, Ho // 2, Wo // 2):
+                raise DvcError(f"{what}: first_last_lab must be [R,3,H/2,W/2]")
+        last = host_or_device((R, 3, Ho // 2, Wo // 2), torch.float32) if return_last else None
+        lam, sigma = (0.0, 1.0) if wls is None else (float(wls[0]), float(wls[1]))
+        ptrs = (ctypes.c_void_p * S)(*[f.data_ptr() for f in clips])
+        optrs = (ctypes.c_void_p * S)(*[o.data_ptr() for o in out])
+        g = (ctypes.c_int * (6 * S))(*geom)
+        rc = self.lib.dvc_colorize_videos_jpeg(self.h, S, ck, ptrs, F_, g, Ho, Wo, float(temperature), _ptr(fl), 0 if wls is None else 1,
+                                               lam, sigma, 1 if source_resolution else 0, int(quality), optrs, out[0].shape[2],
+                                               _ptr(sizes), _ptr(last), _stream(self.device))
+        self._check(rc, f"dvc_{what}")
+        return (out, sizes, last) if return_last else (out, sizes)
+
     # ---- pre / post-processing around the nets (test.py:58,71,100-102) ----------------------------------
     def resize_half(self, x):
         """F.interpolate(x, scale_factor=0.5, mode="bilinear") for a CUDA [B,C,H,W] tensor with even H, W."""
@@ -912,6 +1007,27 @@ def source_footprint(Hs, Ws, Hr, Wr, oy, ox, Ho, Wo):
         raise DvcError(f"dvc_source_footprint failed ({rc}): geometry {(Hs, Ws, Hr, Wr, oy, ox)} has no source pixel inside the "
                        f"{Ho}x{Wo} window, or a size < 1")
     return tuple(fp)
+
+
+def jpeg_max_bytes(h, w):
+    """Upper bound on the size of an h x w JPEG file of encode_jpeg for any content and quality (include/dvc.h:
+    dvc_jpeg_max_bytes).  Needs no GPU."""
+    n = int(load_library().dvc_jpeg_max_bytes(int(h), int(w)))
+    if n < 0:
+        raise DvcError(f"dvc_jpeg_max_bytes failed ({n}): {h}x{w} is outside the encoder's sizes")
+    return n
+
+
+def jpeg_files(slots, sizes):
+    """The files of colorize_videos_jpeg: slots (S tensors [K[s],F,stride]) and sizes [R,F] -> [R][F] lists of bytes, row-major
+    over the clips' rows."""
+    sizes = sizes.cpu()
+    files = []
+    for o in slots:
+        o = o.cpu()
+        for r in range(o.shape[0]):
+            files.append([o[r, t, :int(sizes[len(files), t])].numpy().tobytes() for t in range(o.shape[1])])
+    return files
 
 
 _contexts = {}

@@ -272,6 +272,41 @@ int dvc_colorize_videos_source_rgb8(dvc_ctx* ctx, int S, const int* K, const uns
                                     int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda,
                                     float wls_sigma, unsigned char* const* out, float* last_lab_out, void* stream);
 
+/* ---- JPEG output (test.py:120 writes every frame as a JPEG file) -------------------------------------------------------------
+ * A baseline encoder on the device whose files are byte-identical to Pillow's Image.fromarray(x).save(f, "JPEG", quality=q)
+ * with libjpeg-turbo: 4:2:0 YCbCr (jccolor.c, h2v2_downsample, edge replication), JDCT_ISLOW, jcdctmgr.c's quantizer, the
+ * standard Huffman tables (optimize=False), no restart markers; markers SOI, APP0 JFIF 1.01, DQT luma, DQT chroma, SOF0, DHT
+ * DC/AC luma, DC/AC chroma, SOS, the entropy-coded data, EOI.  Only the finished files leave the device.
+ *
+ * Upper bound on the file size of an H x W image for any content and any quality in [1, 100]:
+ *   623 header bytes + 2 (EOI) + 2 * ceil(1660 * nblocks / 8),  nblocks = 6 ceil(H/16) ceil(W/16)
+ * One block codes a DC difference (code <= 11 bits, value <= 11 bits: category <= 11) and 63 AC coefficients, each a code of
+ * <= 16 bits (the longest standard code) and <= 10 value bits (category <= 10); a ZRL (<= 11 bits) stands for 16 zero
+ * coefficients and an EOB (<= 4 bits) for >= 1, which would otherwise cost <= 26 bits each, so 22 + 63 * 26 = 1660 bits bound a
+ * block; the final byte's 1-bit padding is within the ceil, and 0xFF 0x00 stuffing at most doubles the data.  Needs no context
+ * or device.  DVC_ERR_SHAPE outside H, W in [1, 65535] or for 1660 * nblocks >= 2^31 (about 14 Mpixel). */
+int64_t dvc_jpeg_max_bytes(int H, int W);
+/* dev_rgb [B,H,W,3] uint8 (device) -> B JFIF files at quality `quality` in [1, 100] (jpeg_set_quality(q, force_baseline=TRUE)):
+ * image b's file goes to out + b * stride, its length to sizes[b].  out and sizes may be device memory or page-locked host memory
+ * (on unified addressing the kernels store into it directly, so only the written bytes cross PCIe); pageable host memory is
+ * DVC_ERR_ARG, so are null pointers, B < 1 and a quality outside [1, 100]; stride < dvc_jpeg_max_bytes(H, W) is DVC_ERR_SHAPE.
+ * Seven launches.  Asynchronous on `stream`: sizes and files are valid once it completes. */
+int dvc_encode_jpeg(dvc_ctx* ctx, const unsigned char* dev_rgb, int B, int H, int W, int quality, unsigned char* out, int64_t stride,
+                    int64_t* sizes, void* stream);
+/* The frames of dvc_colorize_videos_exemplars_rgb8 (source_resolution = 0) or of dvc_colorize_videos_source_rgb8 (1), encoded as
+ * dvc_encode_jpeg encodes them: out[s] holds clip s's [K[s],F] slots of `stride` bytes (row r_local of clip s, frame t at
+ * out[s] + (r_local F + t) stride), sizes [R,F] their lengths.  The networks, the recurrence, first_last_lab and last_lab_out
+ * are those of the rgb8 calls, so chunked calls continue a clip exactly.  The encoder runs on the post-processing stream after
+ * Lab -> sRGB of each frame (7 launches per output size: one for the window, one per footprint size) and stores the finished
+ * files straight into their slots; no per-frame host synchronisation, and device memory does not depend on F.  Refuses what the
+ * underlying call refuses, a quality outside [1, 100] or a null out / out[s] / sizes (DVC_ERR_ARG), pageable host memory
+ * (DVC_ERR_ARG) and a stride below dvc_jpeg_max_bytes of the largest output frame (DVC_ERR_SHAPE), before any launch.
+ * Synchronises `stream` before returning. */
+int dvc_colorize_videos_jpeg(dvc_ctx* ctx, int S, const int* K, const unsigned char* const* frames, int F, const int* geom, int Ho,
+                             int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
+                             int source_resolution, int quality, unsigned char* const* out, int64_t stride, int64_t* sizes,
+                             float* last_lab_out, void* stream);
+
 /* ---- pre / post-processing around the nets (SURVEY.md §8f row 1) ------------------------------ */
 
 /* F.interpolate(x, scale_factor=0.5, mode="bilinear") -- test.py:58,71.  dev_src [planes,H,W] (H, W even) ->

@@ -31,8 +31,13 @@ call's last_lab_out.
 network's colour onto the source frame, WLS-filters it against the source frame's own luminance and keeps that luminance.
 The PNGs cover the part of the frame the window covers (dvc_source_footprint): the whole frame unless CenterPad crops it.
 
-What the reference does and this script does not: the AVI writer (folder2vid).  Image decode / encode stays on the host
-(PIL), as in the reference.  Without checkpoints (none ship with the reference tree) pass --seeded-weights to run the
+--format jpg writes <frame>.jpg files instead of PNGs, encoded on the device: every call is dvc_colorize_videos_jpeg (window or,
+with --source-resolution, source output; same chunks, exemplars and recurrence), whose files are byte-equal to Pillow's
+save(f, "JPEG", quality=--jpeg-quality) of the frames the PNG path writes.  Only the compressed files cross PCIe, into a ring of
+pinned slots of dvc_jpeg_max_bytes each (bounded by the chunk size), and the writer threads only write bytes.
+
+What the reference does and this script does not: the AVI writer (folder2vid).  Image decode stays on the host (PIL), as in
+the reference, and so does PNG encoding.  Without checkpoints (none ship with the reference tree) pass --seeded-weights to run the
 pipeline on the seeded random weights of dvc/synth.py (useful as a smoke run only).
 """
 import argparse
@@ -58,6 +63,11 @@ def save_png(img, path):
     from PIL import Image
 
     Image.fromarray(img).save(path)
+
+
+def save_bytes(data, path):
+    with open(path, "wb") as f:
+        f.write(data)
 
 
 class Source:
@@ -117,7 +127,12 @@ def main():
     ap.add_argument("--source-resolution", action="store_true",
                     help="write every frame at its source resolution (the part of the frame the --image-size window covers): the "
                          "network's colour resampled onto the source frame and WLS-filtered against its own luminance")
+    ap.add_argument("--format", choices=("png", "jpg"), default="png",
+                    help="png: Pillow on the host; jpg: baseline JPEG encoded on the device (Pillow's bytes at --jpeg-quality)")
+    ap.add_argument("--jpeg-quality", type=int, default=75, help="JPEG quality in [1, 100] (75: Pillow's default)")
     args = ap.parse_args()
+    if not 1 <= args.jpeg_quality <= 100:
+        raise SystemExit("--jpeg-quality must be in [1, 100]")
     if args.chunk < 1:
         raise SystemExit("--chunk must be >= 1")
     S = len(args.clip)
@@ -216,7 +231,25 @@ def main():
         for f in writes[slot]:  # the encodes of chunk i-2 still read this output slot
             f.result()
         rows = sum(counts[s] for s in active)
-        if args.source_resolution:  # every clip's frames at its footprint, one [K_s,n,h,w,3] buffer per clip
+        if args.format == "jpg":  # the device encodes: one [K_s,n,stride] slot buffer per clip, stride = the largest frame's bound
+            sizes_ = [(H, W)]
+            if args.source_resolution:
+                for chunk in chunks:
+                    Hs, Ws = chunk[0][1].shape[:2]
+                    sizes_.append(dvc.source_footprint(Hs, Ws, *centerpad_geometry(Hs, Ws, (H, W)), H, W)[2:])
+            stride = max(dvc.jpeg_max_bytes(h, w) for h, w in sizes_)
+            shapes = [(counts[s], n, stride) for s in active]
+            if ring_out[slot] is None or [tuple(o.shape) for o in ring_out[slot][0]] != shapes:
+                ring_out[slot] = ([torch.empty(shp, dtype=torch.uint8).pin_memory() for shp in shapes],
+                                  torch.empty(rows, n, dtype=torch.int64).pin_memory())
+            slots, sizes, last = ctx.colorize_videos_jpeg(
+                [ring_in[slot][s][:n] for s in active], [counts[s] for s in active], (H, W), args.jpeg_quality, args.source_resolution,
+                args.temperature, first_last_lab=last, wls=wls, out=ring_out[slot][0], sizes=ring_out[slot][1], return_last=True)
+            files = dvc.jpeg_files(slots, sizes)
+            dests = [(d, chunk) for s, chunk in zip(active, chunks) for d in outs[s]]
+            writes[slot] = [encode.submit(save_bytes, files[r][t], os.path.join(d, os.path.splitext(name)[0] + ".jpg"))
+                            for r, (d, chunk) in enumerate(dests) for t, (name, _) in enumerate(chunk)]
+        elif args.source_resolution:  # every clip's frames at its footprint, one [K_s,n,h,w,3] buffer per clip
             shapes = []
             for chunk in chunks:
                 Hs, Ws = chunk[0][1].shape[:2]
@@ -245,8 +278,9 @@ def main():
                                                            return_last=True)
             dests = [(d, chunk) for s, chunk in zip(active, chunks) for d in outs[s]]
             arr = out.numpy()
-        writes[slot] = [encode.submit(save_png, arr[r][t],os.path.join(d, os.path.splitext(name)[0] + ".png"))
-                        for r, (d, chunk) in enumerate(dests) for t, (name, _) in enumerate(chunk)]
+        if args.format == "png":
+            writes[slot] = [encode.submit(save_png, arr[r][t],os.path.join(d, os.path.splitext(name)[0] + ".png"))
+                            for r, (d, chunk) in enumerate(dests) for t, (name, _) in enumerate(chunk)]
         for s in active:
             done[s] += n
         i += 1
