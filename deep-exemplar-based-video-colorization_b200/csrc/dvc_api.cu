@@ -1915,13 +1915,15 @@ static void rgb_from_xyz(double inv[9]) {
 // ab) exist once.  Nothing depends on F.
 // One frame source per clip: clip s feeds the clip loop's rows of clip s (one row per exemplar of that clip).
 struct VideoSrc {
-  const unsigned char* frames = nullptr;  // [F][Hs][Ws][3], host (pinned) or device
+  const unsigned char* frames = nullptr;  // [F][Hs][Ws][C], host (pinned) or device
+  int C = 3;                              // 3: sRGB frames; 1: grey frames, each byte standing for (g, g, g)
   int Hs = 0, Ws = 0, Hr = 0, Wr = 0, oy = 0, ox = 0;
   int ry = 0, rx = 0, ny = 0, nx = 0;
   size_t tap0 = 0;  // its [wy | wx | 1.0] in VideoIO::taps
   size_t src0 = 0;  // its frame in each of the two source slots
   // source-resolution output (dvc_colorize_videos_source_rgb8): the footprint (y0, x0, h, w), the clip's rows of the clip loop,
-  // its [rows][F][h][w][3] output and its offsets in the source-resolution workspaces
+  // its [rows][F][h][w][3] output and its offsets in the source-resolution workspaces.  The window output of
+  // dvc_colorize_videos_gray8 uses the rows and `out` ([rows][F][Ho][Wo][3]) too.
   int fp[4] = {0, 0, 0, 0};
   int row0 = 0, rows = 1;
   unsigned char* out = nullptr;
@@ -1933,7 +1935,7 @@ struct VideoIO {
   int Ho = 0, Wo = 0;
   bool wls = false;
   float lambda = 0.f, sigma = 0.f;
-  unsigned char* out = nullptr;  // [R][F][Ho][Wo][3] (R rows of the clip loop), host (pinned) or device
+  unsigned char* out = nullptr;  // [R][F][Ho][Wo][3] (R rows of the clip loop), host (pinned) or device; or per clip (VideoSrc)
   float* last_out = nullptr;     // [R][3][Ho/2][Wo/2] or nullptr
   std::vector<double> taps;      // every source's [wy | wx | 1.0]: uploaded once per call
   float lut[256];
@@ -2042,7 +2044,7 @@ static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
   // the source slot was last read by frame t-2's resize
   if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sU, c->evU[(t - 2) & 3], 0));
   for (const VideoSrc& k : v.clips) {
-    const size_t ns = (size_t)k.Hs * k.Ws * 3;
+    const size_t ns = (size_t)k.Hs * k.Ws * k.C;
     CUDA_TRY(c, cudaMemcpyAsync(src + k.src0, k.frames + (size_t)t * ns, ns, cudaMemcpyDefault, c->sU));
   }
   CUDA_TRY(c, cudaEventRecord(c->evR[t & 3], c->sU));
@@ -2057,17 +2059,18 @@ static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
     const size_t plane = (size_t)(t & 3) * S + s;
     // dvc_resize_antialias_crop_rgb8's kernel sequence; a zero-radius "filter" (one tap of weight 1) converts uint8 -> float64
     double *cur = v.f0, *nxt = v.f1;
-    launch_gauss_axis_u8(src + k.src0, cur, k.ny ? taps : taps + k.ny + k.nx, k.ry, 1, k.Hs, k.Ws * 3, c->sI);
+    launch_gauss_axis_u8(src + k.src0, cur, k.ny ? taps : taps + k.ny + k.nx, k.ry, 1, k.Hs, k.Ws * k.C, c->sI);
     if (k.nx) {
-      launch_gauss_axis_f64(cur, nxt, taps + k.ny, k.rx, (size_t)k.Hs, k.Ws, 3, c->sI);
+      launch_gauss_axis_f64(cur, nxt, taps + k.ny, k.rx, (size_t)k.Hs, k.Ws, k.C, c->sI);
       std::swap(cur, nxt);
     }
-    launch_zoom_crop(cur, k.Hs, k.Ws, k.Hr, k.Wr, k.oy, k.ox, v.crop, v.Ho, v.Wo, c->sI);
-    launch_rgb8_to_l_half(v.crop, v.L + plane * hw, Lt + s * (hw / 4), v.wls && !v.source ? v.guide + plane * hw : nullptr, v.Ho, v.Wo,
-                          c->sI);
+    launch_zoom_crop(cur, k.C, k.Hs, k.Ws, k.Hr, k.Wr, k.oy, k.ox, v.crop, v.Ho, v.Wo, c->sI);
+    launch_rgb8_to_l_half(v.crop, k.C, v.L + plane * hw, Lt + s * (hw / 4), v.wls && !v.source ? v.guide + plane * hw : nullptr, v.Ho,
+                          v.Wo, c->sI);
     if (v.source) {  // the source frame's own L and guide over its footprint, while its upload slot is still held
       const size_t sp = (size_t)(t & 3) * v.fp_sum + k.sl0;
-      launch_rgb8_to_l_guide(src + k.src0, k.Ws, k.fp[0], k.fp[1], k.fp[2], k.fp[3], v.sL + sp, v.wls ? v.sguide + sp : nullptr, c->sI);
+      launch_rgb8_to_l_guide(src + k.src0, k.C, k.Ws, k.fp[0], k.fp[1], k.fp[2], k.fp[3], v.sL + sp, v.wls ? v.sguide + sp : nullptr,
+                             c->sI);
     }
   }
   DVC_TRY(check_launch(c, "video ingest"));
@@ -2142,9 +2145,14 @@ static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int
       for (int r = 0; r < k.rows; ++r)
         CUDA_TRY(c, cudaMemcpyAsync(k.out + ((size_t)r * F + t) * n3, srgb + k.srgb0 + r * n3, n3, cudaMemcpyDefault, c->sD));
     }
-  } else {
+  } else if (v.out) {
     for (int r = 0; r < R; ++r)
       CUDA_TRY(c, cudaMemcpyAsync(v.out + ((size_t)r * F + t) * hw * 3, rgb + (size_t)r * hw * 3, hw * 3, cudaMemcpyDefault, c->sD));
+  } else {  // one window output per clip
+    for (const VideoSrc& k : v.clips)
+      for (int r = 0; r < k.rows; ++r)
+        CUDA_TRY(c, cudaMemcpyAsync(k.out + ((size_t)r * F + t) * hw * 3, rgb + (size_t)(k.row0 + r) * hw * 3, hw * 3, cudaMemcpyDefault,
+                                    c->sD));
   }
   CUDA_TRY(c, cudaEventRecord(c->evD[t & 3], c->sD));
   return DVC_OK;
@@ -2306,7 +2314,7 @@ extern "C" int dvc_colorize_clips_exemplars(dvc_ctx* c, const float* L_in, int F
 
 // One frame source of the video calls: geometry g = (Hs, Ws, Hr, Wr, oy, ox) checked as dvc_colorize_video_rgb8 documents
 // it, then appended to v with its anti-aliasing taps
-static int video_add_source(dvc_ctx* c, const char* what, VideoIO& v, const unsigned char* frames, const int g[6]) {
+static int video_add_source(dvc_ctx* c, const char* what, VideoIO& v, const unsigned char* frames, const int g[6], int C = 3) {
   const int Hs = g[0], Ws = g[1], Hr = g[2], Wr = g[3], oy = g[4], ox = g[5];
   if (Hs < 1 || Ws < 1 || Hr < 1 || Wr < 1 || v.Ho < 2 || v.Wo < 2 || (v.Ho & 1) || (v.Wo & 1))
     return fail(c, DVC_ERR_SHAPE, std::string(what) + ": bad geometry (sizes >= 1, an even output size)");
@@ -2314,7 +2322,7 @@ static int video_add_source(dvc_ctx* c, const char* what, VideoIO& v, const unsi
   auto nested = [](int resized, int outsz, int off) { return resized >= outsz ? off >= 0 && off <= resized - outsz : off <= 0 && off >= resized - outsz; };
   if (!nested(Hr, v.Ho, oy) || !nested(Wr, v.Wo, ox)) return fail(c, DVC_ERR_SHAPE, std::string(what) + ": crop offset outside the resized image");
   VideoSrc k;
-  k.frames = frames, k.Hs = Hs, k.Ws = Ws, k.Hr = Hr, k.Wr = Wr, k.oy = oy, k.ox = ox;
+  k.frames = frames, k.C = C, k.Hs = Hs, k.Ws = Ws, k.Hr = Hr, k.Wr = Wr, k.oy = oy, k.ox = ox;
   std::vector<double> wy, wx;
   resize_taps(Hs, Ws, Hr, Wr, &wy, &k.ry, &wx, &k.rx);
   k.ny = (int)wy.size(), k.nx = (int)wx.size();
@@ -2322,7 +2330,7 @@ static int video_add_source(dvc_ctx* c, const char* what, VideoIO& v, const unsi
   v.taps.insert(v.taps.end(), wy.begin(), wy.end());
   v.taps.insert(v.taps.end(), wx.begin(), wx.end());
   v.taps.push_back(1.0);
-  const size_t ns = (size_t)Hs * Ws * 3;
+  const size_t ns = (size_t)Hs * Ws * C;
   k.src0 = v.ns_sum;
   v.ns_sum += ns, v.ns_max = std::max(v.ns_max, ns);
   v.clips.push_back(k);
@@ -2384,6 +2392,18 @@ static int video_source_outputs(dvc_ctx* c, const char* what, VideoIO& v, const 
   return DVC_OK;
 }
 
+// Window output in one buffer per clip: clip s's K[s] rows go to out[s] [K[s]][F][Ho][Wo][3]
+static int video_window_outputs(dvc_ctx* c, const char* what, VideoIO& v, const int* K, unsigned char* const* out) {
+  int row0 = 0;
+  for (size_t s = 0; s < v.clips.size(); ++s) {
+    VideoSrc& k = v.clips[s];
+    if (!out[s]) return fail(c, DVC_ERR_ARG, std::string(what) + ": out[" + std::to_string(s) + "] is null");
+    k.out = out[s], k.row0 = row0, k.rows = K[s];
+    row0 += K[s];
+  }
+  return DVC_OK;
+}
+
 // the checks and settings the video calls share, after their sources: output size, WLS parameters, outputs
 static int video_finish(dvc_ctx* c, const char* what, VideoIO& v, int wls, float wls_lambda, float wls_sigma, unsigned char* out,
                         float* last_lab_out) {
@@ -2411,8 +2431,8 @@ extern "C" int dvc_colorize_video_rgb8(dvc_ctx* c, const unsigned char* frames, 
                             stream, &v);
 }
 
-// S clips, clip s with K[s] exemplar rows (K == nullptr: one each), every clip with its own geometry.  The output is `out` at
-// the window size, or clip s's own source_out[s] at its footprint size (source_out != nullptr; K given then).
+// S clips, clip s with K[s] exemplar rows (K == nullptr: one each), every clip with its own geometry and C channels per pixel.
+// The output is `out` at the window size, clip s's own window_out[s] or source_out[s] at its footprint size (K given for both).
 struct JpegOut {  // dvc_colorize_videos_jpeg's destination
   int quality;
   unsigned char* const* out;
@@ -2424,8 +2444,9 @@ static int video_jpeg_outputs(dvc_ctx* c, const char* what, VideoIO& v, const in
 static int videos_impl(dvc_ctx* c, const char* what, int S, const int* K, const unsigned char* const* frames, int F, const int* geom,
                        int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
                        unsigned char* out, float* last_lab_out, void* stream, unsigned char* const* source_out = nullptr,
-                       const JpegOut* jpeg = nullptr) {
-  if (!c || !frames || !geom || (!out && !source_out && !jpeg) || F < 1) return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
+                       const JpegOut* jpeg = nullptr, int C = 3, unsigned char* const* window_out = nullptr) {
+  if (!c || !frames || !geom || (!out && !source_out && !jpeg && !window_out) || F < 1)
+    return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
   const int* counts = K;
   if (K) {
     DVC_TRY(check_counts(c, what, S, K));
@@ -2437,9 +2458,10 @@ static int videos_impl(dvc_ctx* c, const char* what, int S, const int* K, const 
   v.Ho = Ho, v.Wo = Wo;
   for (int s = 0; s < S; ++s) {
     if (!frames[s]) return fail(c, DVC_ERR_ARG, std::string(what) + ": frames[" + std::to_string(s) + "] is null");
-    DVC_TRY(video_add_source(c, what, v, frames[s], geom + 6 * s));
+    DVC_TRY(video_add_source(c, what, v, frames[s], geom + 6 * s, C));
   }
   DVC_TRY(video_finish(c, what, v, wls, wls_lambda, wls_sigma, out, last_lab_out));
+  if (window_out) DVC_TRY(video_window_outputs(c, what, v, counts, window_out));
   if (source_out) DVC_TRY(video_source_outputs(c, what, v, counts, source_out));
   if (jpeg) DVC_TRY(video_jpeg_outputs(c, what, v, counts, F, *jpeg));
   return colorize_clip_impl(c, what, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, S, K, nullptr, stream, &v);
@@ -2557,6 +2579,27 @@ extern "C" int dvc_colorize_videos_jpeg(dvc_ctx* c, int S, const int* K, const u
   const JpegOut j{quality, out, stride, sizes};
   return videos_impl(c, what, S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda, wls_sigma, nullptr,
                      last_lab_out, stream, source_resolution ? out : nullptr, &j);
+}
+
+// Grey sources: the video calls with one byte per pixel uploaded and resized, and L looked up per byte value; everything after
+// the L planes is the sRGB calls' code
+extern "C" int dvc_colorize_videos_gray8(dvc_ctx* c, int S, const int* K, const unsigned char* const* frames, int F, const int* geom,
+                                         int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda,
+                                         float wls_sigma, int source_resolution, int quality, unsigned char* const* out, int64_t stride,
+                                         int64_t* sizes, float* last_lab_out, void* stream) {
+  const char* what = "colorize_videos_gray8";
+  if (c && !K) return fail(c, DVC_ERR_ARG, std::string(what) + ": K is null");
+  if (c && !out) return fail(c, DVC_ERR_ARG, std::string(what) + ": out is null");
+  if (c && (quality < 0 || quality > 100)) return fail(c, DVC_ERR_ARG, std::string(what) + ": quality must be in [0, 100]");
+  if (quality == 0) {  // sRGB frames
+    if (c && (stride != 0 || sizes)) return fail(c, DVC_ERR_ARG, std::string(what) + ": sRGB output (quality 0) takes stride 0 and no sizes");
+    return videos_impl(c, what, S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda, wls_sigma, nullptr,
+                       last_lab_out, stream, source_resolution ? out : nullptr, nullptr, 1, source_resolution ? nullptr : out);
+  }
+  if (c && !sizes) return fail(c, DVC_ERR_ARG, std::string(what) + ": sizes is null");
+  const JpegOut j{quality, out, stride, sizes};
+  return videos_impl(c, what, S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda, wls_sigma, nullptr,
+                     last_lab_out, stream, source_resolution ? out : nullptr, &j, 1);
 }
 
 extern "C" int dvc_encode_jpeg(dvc_ctx* c, const unsigned char* dev_rgb, int B, int H, int W, int quality, unsigned char* out,
@@ -2745,7 +2788,7 @@ extern "C" int dvc_resize_antialias_crop_rgb8(dvc_ctx* c, const unsigned char* d
     launch_gauss_axis_f64(cur, nxt, (double*)taps + wy.size(), rx, (size_t)Hs, Ws, 3, s);
     std::swap(cur, nxt);
   }
-  launch_zoom_crop(cur, Hs, Ws, Hr, Wr, oy, ox, dev_dst, Ho, Wo, s);
+  launch_zoom_crop(cur, 3, Hs, Ws, Hr, Wr, oy, ox, dev_dst, Ho, Wo, s);
   return check_launch(c, "resize_antialias_crop");
 }
 

@@ -295,12 +295,14 @@ void launch_fgs_horizontal(float* cur, const float* Ch, float* D, int planes, co
 void launch_fgs_vertical(float* cur, const float* Cv, float* D, int planes, const PlaneSrc& gsrc, int H, int W, float lam,
                          cudaStream_t s);
 void launch_l_to_guide8(const float* l, unsigned char* g, size_t n, cudaStream_t s);
-// video ingest: uint8 [H][W][3] (H, W even) -> centred L [H][W] (rgb8_to_lab's plane 0), its 1/2 resolution [H/2][W/2]
-// (resize_half of that plane) and, when guide != nullptr, the WLS guide [H][W] (l_to_guide8 of the L plane)
-void launch_rgb8_to_l_half(const unsigned char* rgb, float* l, float* l_half, unsigned char* guide, int H, int W, cudaStream_t s);
-// source-resolution output of the video path: the footprint (y0, x0, h, w) of a uint8 frame [Hs][Ws][3] -> centred L [h][w]
-// (rgb8_to_lab's plane 0) and, when guide != nullptr, the WLS guide [h][w]
-void launch_rgb8_to_l_guide(const unsigned char* rgb, int Ws, int y0, int x0, int h, int w, float* l, unsigned char* guide, cudaStream_t s);
+// video ingest: uint8 [H][W][C] (H, W even; C = 3 sRGB, or C = 1 grey, read as (g, g, g)) -> centred L [H][W] (rgb8_to_lab's
+// plane 0), its 1/2 resolution [H/2][W/2] (resize_half of that plane) and, when guide != nullptr, the WLS guide [H][W]
+// (l_to_guide8 of the L plane)
+void launch_rgb8_to_l_half(const unsigned char* rgb, int C, float* l, float* l_half, unsigned char* guide, int H, int W, cudaStream_t s);
+// source-resolution output of the video path: the footprint (y0, x0, h, w) of a uint8 frame [Hs][Ws][C] (C as above) -> centred
+// L [h][w] (rgb8_to_lab's plane 0) and, when guide != nullptr, the WLS guide [h][w]
+void launch_rgb8_to_l_guide(const unsigned char* rgb, int C, int Ws, int y0, int x0, int h, int w, float* l, unsigned char* guide,
+                            cudaStream_t s);
 // window ab [planes][Ho][Wo] -> bilinear on the footprint fp = (y0, x0, h, w) of the source grid of geometry g = (Hs, Ws, Hr, Wr,
 // oy, ox): dst [planes][h][w]
 void launch_ab_to_source(const float* ab, int planes, int Ho, int Wo, const int g[6], const int fp[4], float* dst, cudaStream_t s);
@@ -308,7 +310,8 @@ void launch_gauss_axis_u8(const unsigned char* src, double* dst, const double* w
                           cudaStream_t s);
 void launch_gauss_axis_f64(const double* src, double* dst, const double* w, int radius, size_t n_outer, int len, int inner,
                            cudaStream_t s);
-void launch_zoom_crop(const double* src, int Hs, int Ws, int Hr, int Wr, int oy, int ox, unsigned char* dst, int Ho, int Wo,
+// [Hs][Ws][C] float64 (C = 1 or 3) -> [Ho][Wo][C] uint8
+void launch_zoom_crop(const double* src, int C, int Hs, int Ws, int Hr, int Wr, int oy, int ox, unsigned char* dst, int Ho, int Wo,
                       cudaStream_t s);
 
 // Baseline JPEG encoder (jpeg.cu).  Header bytes (SOI .. SOS, identical for every size and quality) and the worst-case bits of

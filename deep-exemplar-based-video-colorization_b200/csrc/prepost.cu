@@ -138,13 +138,29 @@ __global__ void __launch_bounds__(256) l_to_guide8_kernel(const float* __restric
     g[i] = guide8_of_l(__ldg(l + i));
 }
 
+// Centred L of a grey byte g, i.e. of the pixel (g, g, g): rgb8_to_lab_kernel's plane 0 with the same float64 operations
+// (rgb8_lab_f), one entry per byte value, built by each block of the C = 1 ingest kernels before they read it.
+__device__ __forceinline__ void gray_l_table(float* __restrict__ lut) {
+  for (int g = threadIdx.x; g < 256; g += blockDim.x) {
+    const unsigned char px[3] = {(unsigned char)g, (unsigned char)g, (unsigned char)g};
+    double f[3];
+    rgb8_lab_f(px, f);
+    lut[g] = (float)(116.0 * f[1] - 16.0) - 50.0f;
+  }
+  __syncthreads();
+}
+
 // Video ingest (test.py:44-46,71,106 for the luminance only -- the frames' a / b are never used).  A warp owns a 2 x 16
-// pixel tile (lane = row * 16 + column) of the centred uint8 frame, one thread per pixel; the 2 x 2 neighbourhoods of the
-// half-resolution plane are gathered with shuffles.  L is rgb8_to_lab_kernel's plane 0 (the same float64 operations,
-// rgb8_lab_f), the half-resolution value resize_half_kernel's arithmetic on those four floats, the guide l_to_guide8's.
+// pixel tile (lane = row * 16 + column) of the centred uint8 frame [H][W][C], one thread per pixel; the 2 x 2 neighbourhoods
+// of the half-resolution plane are gathered with shuffles.  L is rgb8_to_lab_kernel's plane 0 (the same float64 operations,
+// rgb8_lab_f; for a grey frame, C = 1, looked up in gray_l_table), the half-resolution value resize_half_kernel's arithmetic on
+// those four floats, the guide l_to_guide8's.
+template <int C>
 __global__ void __launch_bounds__(256) rgb8_to_l_half_kernel(const unsigned char* __restrict__ rgb, float* __restrict__ l,
                                                              float* __restrict__ l_half, unsigned char* __restrict__ guide, int H,
                                                              int W) {
+  __shared__ float gray_l[C == 1 ? 256 : 1];
+  if constexpr (C == 1) gray_l_table(gray_l);
   const int lane = threadIdx.x & 31;
   const int tw = (W + 15) / 16, ntiles = (H / 2) * tw, nwarps = gridDim.x * (blockDim.x >> 5);
   for (int tile = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); tile < ntiles; tile += nwarps) {  // warp-uniform
@@ -152,9 +168,13 @@ __global__ void __launch_bounds__(256) rgb8_to_l_half_kernel(const unsigned char
     float v = 0.f;
     if (x < W) {
       const size_t pix = (size_t)y * W + x;
-      double f[3];
-      rgb8_lab_f(rgb + pix * 3, f);
-      v = (float)(116.0 * f[1] - 16.0) - 50.0f;
+      if constexpr (C == 1) {
+        v = gray_l[rgb[pix]];
+      } else {
+        double f[3];
+        rgb8_lab_f(rgb + pix * 3, f);
+        v = (float)(116.0 * f[1] - 16.0) - 50.0f;
+      }
       l[pix] = v;
       if (guide) guide[pix] = guide8_of_l(v);
     }
@@ -167,16 +187,24 @@ __global__ void __launch_bounds__(256) rgb8_to_l_half_kernel(const unsigned char
 }
 
 // Source-resolution luminance of the video path: over the footprint rectangle (y0, x0, h, w) of a uint8 source frame
-// [Hs][Ws][3], the centred L [h][w] (rgb8_to_lab_kernel's plane 0: rgb8_lab_f, the same float64 operations) and, when guide !=
-// nullptr, the WLS guide [h][w] (l_to_guide8's).
+// [Hs][Ws][C], the centred L [h][w] (rgb8_to_lab_kernel's plane 0: rgb8_lab_f, the same float64 operations; gray_l_table for
+// C = 1) and, when guide != nullptr, the WLS guide [h][w] (l_to_guide8's).
+template <int C>
 __global__ void __launch_bounds__(256) rgb8_to_l_guide_kernel(const unsigned char* __restrict__ rgb, int Ws, int y0, int x0, int h, int w,
                                                               float* __restrict__ l, unsigned char* __restrict__ guide) {
+  __shared__ float gray_l[C == 1 ? 256 : 1];
+  if constexpr (C == 1) gray_l_table(gray_l);
   const size_t n = (size_t)h * w;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const int y = (int)(i / w), x = (int)(i - (size_t)y * w);
-    double f[3];
-    rgb8_lab_f(rgb + ((size_t)(y0 + y) * Ws + x0 + x) * 3, f);
-    const float v = (float)(116.0 * f[1] - 16.0) - 50.0f;
+    float v;
+    if constexpr (C == 1) {
+      v = gray_l[rgb[(size_t)(y0 + y) * Ws + x0 + x]];
+    } else {
+      double f[3];
+      rgb8_lab_f(rgb + ((size_t)(y0 + y) * Ws + x0 + x) * 3, f);
+      v = (float)(116.0 * f[1] - 16.0) - 50.0f;
+    }
     l[i] = v;
     if (guide) guide[i] = guide8_of_l(v);
   }
@@ -242,15 +270,16 @@ __global__ void __launch_bounds__(256) gauss_axis_kernel(const TIn* __restrict__
   }
 }
 
-// scipy.ndimage.zoom(order=1, mode="mirror", grid_mode=True) of a [Hs][Ws][3] float64 image to [Hr][Wr], truncated to
+// scipy.ndimage.zoom(order=1, mode="mirror", grid_mode=True) of a [Hs][Ws][C] float64 image to [Hr][Wr], truncated to
 // uint8 (ndarray.astype(np.uint8) of in-range values), then CenterPad's centred crop (offset oy, ox) / zero pad into
-// the [Ho][Wo][3] output.
+// the [Ho][Wo][C] output.  Channels are independent: a grey frame (C = 1) gives each channel of its (g, g, g) expansion.
+template <int C>
 __global__ void __launch_bounds__(256) zoom_crop_kernel(const double* __restrict__ src, int Hs, int Ws, int Hr, int Wr, int oy, int ox,
                                                         unsigned char* __restrict__ dst, int Ho, int Wo) {
-  const size_t total = (size_t)Ho * Wo * 3;
+  const size_t total = (size_t)Ho * Wo * C;
   for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
-    const int ch = (int)(idx % 3);
-    const size_t t = idx / 3;
+    const int ch = (int)(idx % C);
+    const size_t t = idx / C;
     const int xo = (int)(t % Wo), yo = (int)(t / Wo);
     const int yr = yo + oy, xr = xo + ox;  // position in the resized image
     unsigned char out = 0;
@@ -263,8 +292,8 @@ __global__ void __launch_bounds__(256) zoom_crop_kernel(const double* __restrict
       const double ty = __dsub_rn(cy, fy), tx = __dsub_rn(cx, fx);
       const int y0 = mirror_idx((int)fy, Hs), y1 = mirror_idx((int)fy + 1, Hs);
       const int x0 = mirror_idx((int)fx, Ws), x1 = mirror_idx((int)fx + 1, Ws);
-      const double v00 = src[((size_t)y0 * Ws + x0) * 3 + ch], v01 = src[((size_t)y0 * Ws + x1) * 3 + ch];
-      const double v10 = src[((size_t)y1 * Ws + x0) * 3 + ch], v11 = src[((size_t)y1 * Ws + x1) * 3 + ch];
+      const double v00 = src[((size_t)y0 * Ws + x0) * C + ch], v01 = src[((size_t)y0 * Ws + x1) * C + ch];
+      const double v10 = src[((size_t)y1 * Ws + x0) * C + ch], v11 = src[((size_t)y1 * Ws + x1) * C + ch];
       // scipy (ni_interpolation.c) sums the 2 x 2 neighbourhood, row-major, each term ((value * wy) * wx)
       const double wy0 = __dsub_rn(1.0, ty), wx0 = __dsub_rn(1.0, tx);
       double v = __dmul_rn(__dmul_rn(v00, wy0), wx0);
@@ -394,12 +423,20 @@ void launch_l_to_guide8(const float* l, unsigned char* g, size_t n, cudaStream_t
   l_to_guide8_kernel<<<grid_for(n, 256), 256, 0, s>>>(l, g, n);
   launch_counter_add(1);
 }
-void launch_rgb8_to_l_half(const unsigned char* rgb, float* l, float* l_half, unsigned char* guide, int H, int W, cudaStream_t s) {
-  rgb8_to_l_half_kernel<<<grid_for((size_t)(H / 2) * ((W + 15) / 16) * 32, 256), 256, 0, s>>>(rgb, l, l_half, guide, H, W);
+void launch_rgb8_to_l_half(const unsigned char* rgb, int C, float* l, float* l_half, unsigned char* guide, int H, int W, cudaStream_t s) {
+  const int grid = grid_for((size_t)(H / 2) * ((W + 15) / 16) * 32, 256);
+  if (C == 1)
+    rgb8_to_l_half_kernel<1><<<grid, 256, 0, s>>>(rgb, l, l_half, guide, H, W);
+  else
+    rgb8_to_l_half_kernel<3><<<grid, 256, 0, s>>>(rgb, l, l_half, guide, H, W);
   launch_counter_add(1);
 }
-void launch_rgb8_to_l_guide(const unsigned char* rgb, int Ws, int y0, int x0, int h, int w, float* l, unsigned char* guide, cudaStream_t s) {
-  rgb8_to_l_guide_kernel<<<grid_for((size_t)h * w, 256), 256, 0, s>>>(rgb, Ws, y0, x0, h, w, l, guide);
+void launch_rgb8_to_l_guide(const unsigned char* rgb, int C, int Ws, int y0, int x0, int h, int w, float* l, unsigned char* guide,
+                            cudaStream_t s) {
+  if (C == 1)
+    rgb8_to_l_guide_kernel<1><<<grid_for((size_t)h * w, 256), 256, 0, s>>>(rgb, Ws, y0, x0, h, w, l, guide);
+  else
+    rgb8_to_l_guide_kernel<3><<<grid_for((size_t)h * w, 256), 256, 0, s>>>(rgb, Ws, y0, x0, h, w, l, guide);
   launch_counter_add(1);
 }
 void launch_ab_to_source(const float* ab, int planes, int Ho, int Wo, const int g[6], const int fp[4], float* dst, cudaStream_t s) {
@@ -417,9 +454,12 @@ void launch_gauss_axis_f64(const double* src, double* dst, const double* w, int 
   gauss_axis_kernel<double><<<grid_for(n_outer * len * inner, 256), 256, 0, s>>>(src, dst, w, radius, n_outer, len, inner);
   launch_counter_add(1);
 }
-void launch_zoom_crop(const double* src, int Hs, int Ws, int Hr, int Wr, int oy, int ox, unsigned char* dst, int Ho, int Wo,
+void launch_zoom_crop(const double* src, int C, int Hs, int Ws, int Hr, int Wr, int oy, int ox, unsigned char* dst, int Ho, int Wo,
                       cudaStream_t s) {
-  zoom_crop_kernel<<<grid_for((size_t)Ho * Wo * 3, 256), 256, 0, s>>>(src, Hs, Ws, Hr, Wr, oy, ox, dst, Ho, Wo);
+  if (C == 1)
+    zoom_crop_kernel<1><<<grid_for((size_t)Ho * Wo, 256), 256, 0, s>>>(src, Hs, Ws, Hr, Wr, oy, ox, dst, Ho, Wo);
+  else
+    zoom_crop_kernel<3><<<grid_for((size_t)Ho * Wo * 3, 256), 256, 0, s>>>(src, Hs, Ws, Hr, Wr, oy, ox, dst, Ho, Wo);
   launch_counter_add(1);
 }
 

@@ -32,7 +32,7 @@ EXPORTED = [
     "dvc_corr_softmax_warp_exemplars", "dvc_colorize_video_rgb8", "dvc_colorize_frames_clips", "dvc_colorize_clips",
     "dvc_colorize_videos_rgb8", "dvc_colorize_frames_clips_exemplars", "dvc_colorize_clips_exemplars",
     "dvc_colorize_videos_exemplars_rgb8", "dvc_source_footprint", "dvc_ab_to_source", "dvc_colorize_videos_source_rgb8",
-    "dvc_jpeg_max_bytes", "dvc_encode_jpeg", "dvc_colorize_videos_jpeg",
+    "dvc_jpeg_max_bytes", "dvc_encode_jpeg", "dvc_colorize_videos_jpeg", "dvc_colorize_videos_gray8",
 ]
 
 _lib = None
@@ -102,6 +102,7 @@ def load_library():
         lib.dvc_encode_jpeg.argtypes = [c_void, c_void, c_int, c_int, c_int, c_int, c_void, c_i64, c_void, c_void]
         lib.dvc_colorize_videos_jpeg.argtypes = [c_void, c_int, P(c_int), P(c_void), c_int, P(c_int), c_int, c_int, c_float, c_void,
                                                  c_int, c_float, c_float, c_int, c_int, P(c_void), c_i64, c_void, c_void, c_void]
+        lib.dvc_colorize_videos_gray8.argtypes = lib.dvc_colorize_videos_jpeg.argtypes
         lib.dvc_exemplar_pack_size.argtypes = [c_void, c_int, c_int]
         lib.dvc_exemplar_pack_size.restype = c_i64
         lib.dvc_exemplar_export.argtypes = [c_void, c_void, c_i64, c_void]
@@ -772,6 +773,89 @@ class Context:
                                                _ptr(sizes), _ptr(last), _stream(self.device))
         self._check(rc, f"dvc_{what}")
         return (out, sizes, last) if return_last else (out, sizes)
+
+    # ---- greyscale sources: one byte per pixel in, the sRGB calls' bytes out ------------------------------------------------------
+    def colorize_videos_gray8(self, clips, K, size, temperature=1e-10, first_last_lab=None, wls=(500.0, 4.0), source_resolution=False,
+                              quality=None, out=None, sizes=None, return_last=False):
+        """The video calls for grey clips (include/dvc.h: dvc_colorize_videos_gray8): clips is a list of S uint8 tensors [F,Hs,Ws]
+        (or [F,Hs,Ws,1]).  Returns exactly what the matching call returns for the clips with each byte repeated into R, G and B:
+        colorize_videos_exemplars_rgb8 (window output), colorize_videos_source_rgb8 (source_resolution=True) or, when quality is
+        given, colorize_videos_jpeg.  `out` / `sizes` are those calls' output arguments."""
+        from dvc.prepost import centerpad_geometry
+
+        what = "colorize_videos_gray8"
+        clips = list(clips)
+        if not clips or not all(isinstance(f, torch.Tensor) and f.dtype == torch.uint8 and (f.dim() == 3 or (f.dim() == 4 and f.shape[3] == 1))
+                                for f in clips):
+            raise DvcError(f"{what}: expected a list of uint8 tensors [F,Hs,Ws] (or [F,Hs,Ws,1])")
+        clips = [f[..., 0] if f.dim() == 4 else f for f in clips]
+        on_device = clips[0].is_cuda
+        if any(f.is_cuda != on_device for f in clips) or len({f.shape[0] for f in clips}) != 1:
+            raise DvcError(f"{what}: the clips must have the same frame count and all live on the host or all on the device")
+        clips = [f.contiguous() for f in clips]
+        if not on_device:
+            clips = [f if f.is_pinned() else f.pin_memory() for f in clips]
+        S, F_ = len(clips), clips[0].shape[0]
+        K, ck = self._counts(K, S, what)
+        R = sum(K)
+        Ho, Wo = int(size[0]), int(size[1])
+        geom, frame_sizes = [], []
+        for f in clips:
+            g = [f.shape[1], f.shape[2], *centerpad_geometry(f.shape[1], f.shape[2], (Ho, Wo))]
+            geom += g
+            frame_sizes.append(tuple(source_footprint(*g, Ho, Wo)[2:]) if source_resolution else (Ho, Wo))
+
+        def host_or_device(shape, dtype):
+            t = torch.empty(*shape, dtype=dtype, device=clips[0].device)
+            return t if on_device else t.pin_memory()
+
+        if quality is not None:  # colorize_videos_jpeg's slots and sizes
+            stride = max(jpeg_max_bytes(h, w) for h, w in frame_sizes + [(Ho, Wo)])
+            if out is None:
+                out = [host_or_device((k, F_, stride), torch.uint8) for k in K]
+            out = list(out)
+            if len(out) != S or any(o.dtype != torch.uint8 or not o.is_contiguous() or o.dim() != 3 or tuple(o.shape[:2]) != (k, F_)
+                                    for o, k in zip(out, K)) or len({o.shape[2] for o in out}) != 1:
+                raise DvcError(f"{what}: `out` must be a list of contiguous uint8 [K[s],F,stride] tensors with one stride")
+            if sizes is None:
+                sizes = host_or_device((R, F_), torch.int64)
+            if sizes.dtype != torch.int64 or not sizes.is_contiguous() or tuple(sizes.shape) != (R, F_):
+                raise DvcError(f"{what}: sizes must be a contiguous int64 [R,F] tensor")
+            per_clip, stride = out, out[0].shape[2]
+        elif source_resolution:  # colorize_videos_source_rgb8's list of footprint-size clips
+            shapes = [(k, F_, h, w, 3) for k, (h, w) in zip(K, frame_sizes)]
+            if out is None:
+                out = [host_or_device(shp, torch.uint8) for shp in shapes]
+            out = list(out)
+            if len(out) != S or any(o.is_cuda != on_device or o.dtype != torch.uint8 or not o.is_contiguous() or tuple(o.shape) != shp
+                                    for o, shp in zip(out, shapes)):
+                raise DvcError(f"{what}: `out` must be a list of contiguous uint8 [K[s],F,h_s,w_s,3] tensors (the footprints) on the "
+                               "same side as the clips")
+            per_clip, stride = out, 0
+        else:  # colorize_videos_exemplars_rgb8's [R,F,Ho,Wo,3], handed over clip by clip
+            if out is None:
+                out = host_or_device((R, F_, Ho, Wo, 3), torch.uint8)
+            if (out.is_cuda != on_device or out.dtype != torch.uint8 or not out.is_contiguous()
+                    or tuple(out.shape) != (R, F_, Ho, Wo, 3)):
+                raise DvcError(f"{what}: `out` must be a contiguous uint8 [R,F,H,W,3] tensor on the same side as the clips")
+            per_clip, stride = list(torch.split(out, K)), 0
+        fl = None
+        if first_last_lab is not None:
+            fl = first_last_lab.to(torch.float32).contiguous()
+            if tuple(fl.shape) != (R, 3, Ho // 2, Wo // 2):
+                raise DvcError(f"{what}: first_last_lab must be [R,3,H/2,W/2]")
+        last = host_or_device((R, 3, Ho // 2, Wo // 2), torch.float32) if return_last else None
+        lam, sigma = (0.0, 1.0) if wls is None else (float(wls[0]), float(wls[1]))
+        ptrs = (ctypes.c_void_p * S)(*[f.data_ptr() for f in clips])
+        optrs = (ctypes.c_void_p * S)(*[o.data_ptr() for o in per_clip])
+        g = (ctypes.c_int * (6 * S))(*geom)
+        rc = self.lib.dvc_colorize_videos_gray8(self.h, S, ck, ptrs, F_, g, Ho, Wo, float(temperature), _ptr(fl), 0 if wls is None else 1,
+                                                lam, sigma, 1 if source_resolution else 0, 0 if quality is None else int(quality), optrs,
+                                                stride, _ptr(sizes if quality is not None else None), _ptr(last), _stream(self.device))
+        self._check(rc, f"dvc_{what}")
+        res = (out, sizes) if quality is not None else (out,)
+        res += (last,) if return_last else ()
+        return res if len(res) > 1 else res[0]
 
     # ---- pre / post-processing around the nets (test.py:58,71,100-102) ----------------------------------
     def resize_half(self, x):

@@ -307,6 +307,24 @@ int dvc_colorize_videos_jpeg(dvc_ctx* ctx, int S, const int* K, const unsigned c
                              int source_resolution, int quality, unsigned char* const* out, int64_t stride, int64_t* sizes,
                              float* last_lab_out, void* stream);
 
+/* ---- greyscale sources -------------------------------------------------------------------------------------------------------
+ * The video calls for single-channel frames: frames[s] is clip s's [F,Hs_s,Ws_s] uint8 (one byte per pixel), host-pinned or
+ * device memory; K, geom, the rows, the recurrence, first_last_lab and last_lab_out are as in dvc_colorize_videos_exemplars_rgb8,
+ * and exemplars stay colour images (dvc_set_exemplar(s)).
+ *   quality == 0: out[s] receives clip s's sRGB frames [K[s],F,h,w,3], (h, w) the window (Ho, Wo), or the footprint
+ *                 (dvc_source_footprint) when source_resolution is set; stride must be 0 and sizes NULL.
+ *   quality in [1, 100]: out, stride and sizes are exactly dvc_colorize_videos_jpeg's.
+ * Contract: every output byte (and, for JPEG, every size) and last_lab_out equal what the corresponding sRGB call --
+ * dvc_colorize_videos_exemplars_rgb8 (with its [R,F,Ho,Wo,3] rows split by clip), dvc_colorize_videos_source_rgb8 or
+ * dvc_colorize_videos_jpeg -- returns for the frames with each byte g replicated into (g, g, g).  Only Hs Ws bytes per frame
+ * are uploaded and resized, and L is looked up per byte value; the launches per frame step are those of that call.  Refuses
+ * what that call refuses, plus a null out / out[s], a quality outside [0, 100], and quality == 0 with a non-zero stride or a
+ * non-null sizes (DVC_ERR_ARG), before any launch.  Synchronises `stream` before returning. */
+int dvc_colorize_videos_gray8(dvc_ctx* ctx, int S, const int* K, const unsigned char* const* frames, int F, const int* geom, int Ho,
+                              int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
+                              int source_resolution, int quality, unsigned char* const* out, int64_t stride, int64_t* sizes,
+                              float* last_lab_out, void* stream);
+
 /* ---- pre / post-processing around the nets (SURVEY.md §8f row 1) ------------------------------ */
 
 /* F.interpolate(x, scale_factor=0.5, mode="bilinear") -- test.py:58,71.  dev_src [planes,H,W] (H, W even) ->

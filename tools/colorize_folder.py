@@ -36,6 +36,12 @@ with --source-resolution, source output; same chunks, exemplars and recurrence),
 save(f, "JPEG", quality=--jpeg-quality) of the frames the PNG path writes.  Only the compressed files cross PCIe, into a ring of
 pinned slots of dvc_jpeg_max_bytes each (bounded by the chunk size), and the writer threads only write bytes.
 
+Grey frames (mode "L" images) are decoded as one byte per pixel.  A call whose clips are all grey is
+dvc_colorize_videos_gray8 (every --format, with or without --source-resolution), which uploads and resizes a third of the
+bytes and writes what the sRGB calls write for the frames converted to RGB; a call that mixes grey and colour clips expands
+the grey frames to RGB on the host.  A folder that changes between grey and colour splits its chunks there, like a change of
+size.  Output names and bytes do not depend on which path a frame took.
+
 What the reference does and this script does not: the AVI writer (folder2vid).  Image decode stays on the host (PIL), as in
 the reference, and so does PNG encoding.  Without checkpoints (none ship with the reference tree) pass --seeded-weights to run the
 pipeline on the seeded random weights of dvc/synth.py (useful as a smoke run only).
@@ -57,6 +63,14 @@ def load_rgb8(path):
     from PIL import Image
 
     return np.asarray(Image.open(path).convert("RGB"), dtype=np.uint8)
+
+
+def load_frame(path):
+    """A mode-"L" (8-bit grey) image as [H,W], anything else converted to sRGB [H,W,3]."""
+    from PIL import Image
+
+    img = Image.open(path)
+    return np.asarray(img if img.mode == "L" else img.convert("RGB"), dtype=np.uint8)
 
 
 def save_png(img, path):
@@ -81,12 +95,13 @@ class Source:
 
     def read_ahead(self):
         for n in self.todo:
-            self.pending.append((n, self.decode.submit(load_rgb8, os.path.join(self.folder, n))))
+            self.pending.append((n, self.decode.submit(load_frame, os.path.join(self.folder, n))))
             if len(self.pending) >= 2 * self.chunk:
                 break
 
     def run(self):
-        """Number of decoded frames of one source size at the front, up to the chunk size (0: the clip is done)."""
+        """Number of decoded frames of one source shape (size and grey / colour) at the front, up to the chunk size (0: the clip
+        is done)."""
         self.read_ahead()
         n = 0
         while n < min(self.chunk, len(self.pending)):
@@ -222,15 +237,20 @@ def main():
             ctx.set_exemplars(torch.cat([ref_lab[s] for s in active]))
         n, slot = min(runs), i & 1
         chunks = [sources[s].take(n) for s in active]
+        # grey frames ([H,W], mode "L") go up one byte per pixel when every clip of the call is grey; beside colour clips they
+        # are expanded to (g, g, g) here, which is what the grey call computes anyway
+        gray = all(chunk[0][1].ndim == 2 for chunk in chunks)
         for s, chunk in zip(active, chunks):
-            shape = chunk[0][1].shape
+            shape = chunk[0][1].shape[:2] + (() if gray else (3,))
             if ring_in[slot][s] is None or tuple(ring_in[slot][s].shape[1:]) != shape:
                 ring_in[slot][s] = torch.empty((C,) + shape, dtype=torch.uint8).pin_memory()
             for t, (_, img) in enumerate(chunk):
-                ring_in[slot][s][t].copy_(torch.from_numpy(img))
+                src = torch.from_numpy(img)
+                ring_in[slot][s][t].copy_(src if src.dim() == len(shape) else src[..., None])  # [H,W,1] broadcasts to [H,W,3]
         for f in writes[slot]:  # the encodes of chunk i-2 still read this output slot
             f.result()
         rows = sum(counts[s] for s in active)
+        ins, ks = [ring_in[slot][s][:n] for s in active], [counts[s] for s in active]
         if args.format == "jpg":  # the device encodes: one [K_s,n,stride] slot buffer per clip, stride = the largest frame's bound
             sizes_ = [(H, W)]
             if args.source_resolution:
@@ -242,9 +262,13 @@ def main():
             if ring_out[slot] is None or [tuple(o.shape) for o in ring_out[slot][0]] != shapes:
                 ring_out[slot] = ([torch.empty(shp, dtype=torch.uint8).pin_memory() for shp in shapes],
                                   torch.empty(rows, n, dtype=torch.int64).pin_memory())
-            slots, sizes, last = ctx.colorize_videos_jpeg(
-                [ring_in[slot][s][:n] for s in active], [counts[s] for s in active], (H, W), args.jpeg_quality, args.source_resolution,
-                args.temperature, first_last_lab=last, wls=wls, out=ring_out[slot][0], sizes=ring_out[slot][1], return_last=True)
+            kw = dict(first_last_lab=last, wls=wls, out=ring_out[slot][0], sizes=ring_out[slot][1], return_last=True)
+            if gray:
+                slots, sizes, last = ctx.colorize_videos_gray8(ins, ks, (H, W), args.temperature, source_resolution=args.source_resolution,
+                                                               quality=args.jpeg_quality, **kw)
+            else:
+                slots, sizes, last = ctx.colorize_videos_jpeg(ins, ks, (H, W), args.jpeg_quality, args.source_resolution, args.temperature,
+                                                              **kw)
             files = dvc.jpeg_files(slots, sizes)
             dests = [(d, chunk) for s, chunk in zip(active, chunks) for d in outs[s]]
             writes[slot] = [encode.submit(save_bytes, files[r][t], os.path.join(d, os.path.splitext(name)[0] + ".jpg"))
@@ -258,11 +282,20 @@ def main():
             shapes = [(counts[s], n, h, w, 3) for s, (h, w) in zip(active, shapes)]
             if ring_out[slot] is None or [tuple(o.shape) for o in ring_out[slot]] != shapes:
                 ring_out[slot] = [torch.empty(shp, dtype=torch.uint8).pin_memory() for shp in shapes]
-            res, last = ctx.colorize_videos_source_rgb8([ring_in[slot][s][:n] for s in active], [counts[s] for s in active], (H, W),
-                                                        args.temperature, first_last_lab=last, wls=wls, out=ring_out[slot],
-                                                        return_last=True)
+            kw = dict(first_last_lab=last, wls=wls, out=ring_out[slot], return_last=True)
+            if gray:
+                res, last = ctx.colorize_videos_gray8(ins, ks, (H, W), args.temperature, source_resolution=True, **kw)
+            else:
+                res, last = ctx.colorize_videos_source_rgb8(ins, ks, (H, W), args.temperature, **kw)
             arr = [row for o in res for row in o.numpy()]
             dests = [(d, chunk) for s, chunk in zip(active, chunks) for d in outs[s]]
+        elif gray:  # window output of grey clips, one or several
+            if ring_out[slot] is None or tuple(ring_out[slot].shape[:2]) != (rows, n):
+                ring_out[slot] = torch.empty(rows, n, H, W, 3, dtype=torch.uint8).pin_memory()
+            out, last = ctx.colorize_videos_gray8(ins, ks, (H, W), args.temperature, first_last_lab=last, wls=wls, out=ring_out[slot],
+                                                  return_last=True)
+            dests = [(d, chunk) for s, chunk in zip(active, chunks) for d in outs[s]]
+            arr = out.numpy()
         elif S == 1:
             if ring_out[slot] is None or tuple(ring_out[slot].shape[:2]) != (rows, n):
                 ring_out[slot] = torch.empty(rows, n, H, W, 3, dtype=torch.uint8).pin_memory()
