@@ -1914,9 +1914,14 @@ static void rgb_from_xyz(double inv[9]) {
 // stage run in order on one stream, so the stage's scratch buffers (fp64 resize planes, crop, FGS Ch / Cv / D, up-sampled
 // ab) exist once.  Nothing depends on F.
 // One frame source per clip: clip s feeds the clip loop's rows of clip s (one row per exemplar of that clip).
+// I420 frames are converted to sRGB (cv2's COLOR_YUV2RGB_I420) into one staging frame on stream I, which the sRGB kernel
+// sequence then reads: the clips are ingested one after another, so one staging frame of the largest clip serves them all.
+enum class SrcFormat { RGB8, GRAY8, I420 };
 struct VideoSrc {
-  const unsigned char* frames = nullptr;  // [F][Hs][Ws][C], host (pinned) or device
-  int C = 3;                              // 3: sRGB frames; 1: grey frames, each byte standing for (g, g, g)
+  const unsigned char* frames = nullptr;  // [F][Hs][Ws][C] (RGB8, GRAY8) or [F][3Hs/2][Ws] (I420), host (pinned) or device
+  SrcFormat fmt = SrcFormat::RGB8;
+  int C = 3;                              // channels the resize reads: 3 (sRGB or staged I420); 1: grey, each byte standing for (g, g, g)
+  size_t ns = 0;                          // bytes of one uploaded frame
   int Hs = 0, Ws = 0, Hr = 0, Wr = 0, oy = 0, ox = 0;
   int ry = 0, rx = 0, ny = 0, nx = 0;
   size_t tap0 = 0;  // its [wy | wx | 1.0] in VideoIO::taps
@@ -1931,7 +1936,11 @@ struct VideoSrc {
 };
 struct VideoIO {
   std::vector<VideoSrc> clips;    // S sources
-  size_t ns_sum = 0, ns_max = 0;  // bytes of one frame of all sources / of the largest
+  size_t ns_sum = 0, ns_max = 0;  // bytes of one uploaded frame of all sources / samples of the largest resize plane
+  size_t stage_max = 0;           // bytes of the largest I420 clip's staged sRGB frame (0: no I420 clip)
+  // I420 output (dvc_colorize_videos_i420 with out_i420): the sRGB slot of every output size converted (cv2's
+  // COLOR_RGB2YUV_I420) into two I420 ring slots, 1.5 bytes per pixel, which stream D downloads
+  bool out_i420 = false;
   int Ho = 0, Wo = 0;
   bool wls = false;
   float lambda = 0.f, sigma = 0.f;
@@ -1961,7 +1970,7 @@ struct VideoIO {
   std::vector<std::vector<int>> groups;
   size_t fp_sum = 0, fp_rows = 0, fp_max = 0, fp_rows_max = 0;
   // device workspaces
-  unsigned char *src = nullptr, *crop = nullptr, *guide = nullptr, *rgb = nullptr;
+  unsigned char *src = nullptr, *crop = nullptr, *guide = nullptr, *rgb = nullptr, *stage = nullptr, *yuv = nullptr;
   double *f0 = nullptr, *f1 = nullptr, *dtaps = nullptr;
   float *dlut = nullptr, *L = nullptr, *abL = nullptr, *Ch = nullptr, *Cv = nullptr, *D = nullptr;
   float *sL = nullptr, *sab = nullptr;
@@ -1997,12 +2006,14 @@ static int video_prologue(dvc_ctx* c, VideoIO& v, int R, cudaStream_t s) {
   DVC_TRY(raw("f1", v.ns_max * 8, &v.f1));
   DVC_TRY(raw("taps", v.taps.size() * 8, &v.dtaps));
   DVC_TRY(raw("crop", hw * 3, &v.crop));
+  if (v.stage_max) DVC_TRY(raw("stage", v.stage_max, &v.stage));
   DVC_TRY(raw("L", 4 * S * hw * 4, &v.L));  // 4 slots, like the half-resolution L of the clip loop
   DVC_TRY(raw("abL", (size_t)R * 2 * hw * 4, &v.abL));
   if (v.source) {  // the source-resolution L and guide in 4 slots like v.L, the resampled ab, 2 rgb slots
     DVC_TRY(raw("sL", 4 * v.fp_sum * 4, &v.sL));
     DVC_TRY(raw("sab", v.fp_rows * 2 * 4, &v.sab));
     DVC_TRY(raw("srgb", 2 * v.fp_rows * 3, &v.srgb));
+    if (v.out_i420) DVC_TRY(raw("syuv", 2 * v.fp_rows * 3 / 2, &v.yuv));
     if (v.wls) {
       DVC_TRY(raw("sguide", 4 * v.fp_sum, &v.sguide));
       DVC_TRY(raw("lut", 256 * 4, &v.dlut));
@@ -2013,6 +2024,7 @@ static int video_prologue(dvc_ctx* c, VideoIO& v, int R, cudaStream_t s) {
     }
   } else {
     DVC_TRY(raw("rgb", 2 * (size_t)R * hw * 3, &v.rgb));  // 2 slots
+    if (v.out_i420) DVC_TRY(raw("yuv", 2 * (size_t)R * hw * 3 / 2, &v.yuv));
     if (v.wls) {
       DVC_TRY(raw("guide", 4 * S * hw, &v.guide));  // 4 slots
       DVC_TRY(raw("lut", 256 * 4, &v.dlut));
@@ -2043,10 +2055,8 @@ static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
   unsigned char* src = v.src + (size_t)(t & 1) * v.ns_sum;
   // the source slot was last read by frame t-2's resize
   if (t >= 2) CUDA_TRY(c, cudaStreamWaitEvent(c->sU, c->evU[(t - 2) & 3], 0));
-  for (const VideoSrc& k : v.clips) {
-    const size_t ns = (size_t)k.Hs * k.Ws * k.C;
-    CUDA_TRY(c, cudaMemcpyAsync(src + k.src0, k.frames + (size_t)t * ns, ns, cudaMemcpyDefault, c->sU));
-  }
+  for (const VideoSrc& k : v.clips)
+    CUDA_TRY(c, cudaMemcpyAsync(src + k.src0, k.frames + (size_t)t * k.ns, k.ns, cudaMemcpyDefault, c->sU));
   CUDA_TRY(c, cudaEventRecord(c->evR[t & 3], c->sU));
   // the half-resolution L slot was last read by frame t-4's ColorVidNet / make_last, the full-resolution L and guide slots
   // by frame t-4's post-processing
@@ -2057,9 +2067,14 @@ static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
     const VideoSrc& k = v.clips[s];
     const double* taps = v.dtaps + k.tap0;
     const size_t plane = (size_t)(t & 3) * S + s;
+    const unsigned char* frame = src + k.src0;
+    if (k.fmt == SrcFormat::I420) {
+      launch_i420_to_rgb8(frame, v.stage, 1, k.Hs, k.Ws, c->sI);
+      frame = v.stage;
+    }
     // dvc_resize_antialias_crop_rgb8's kernel sequence; a zero-radius "filter" (one tap of weight 1) converts uint8 -> float64
     double *cur = v.f0, *nxt = v.f1;
-    launch_gauss_axis_u8(src + k.src0, cur, k.ny ? taps : taps + k.ny + k.nx, k.ry, 1, k.Hs, k.Ws * k.C, c->sI);
+    launch_gauss_axis_u8(frame, cur, k.ny ? taps : taps + k.ny + k.nx, k.ry, 1, k.Hs, k.Ws * k.C, c->sI);
     if (k.nx) {
       launch_gauss_axis_f64(cur, nxt, taps + k.ny, k.rx, (size_t)k.Hs, k.Ws, k.C, c->sI);
       std::swap(cur, nxt);
@@ -2069,7 +2084,7 @@ static int video_ingest(dvc_ctx* c, const VideoIO& v, int t, float* Lt) {
                           v.Wo, c->sI);
     if (v.source) {  // the source frame's own L and guide over its footprint, while its upload slot is still held
       const size_t sp = (size_t)(t & 3) * v.fp_sum + k.sl0;
-      launch_rgb8_to_l_guide(src + k.src0, k.C, k.Ws, k.fp[0], k.fp[1], k.fp[2], k.fp[3], v.sL + sp, v.wls ? v.sguide + sp : nullptr,
+      launch_rgb8_to_l_guide(frame, k.C, k.Ws, k.fp[0], k.fp[1], k.fp[2], k.fp[3], v.sL + sp, v.wls ? v.sguide + sp : nullptr,
                              c->sI);
     }
   }
@@ -2102,6 +2117,7 @@ static void video_post_source(const VideoIO& v, int t, const double inv[9], cuda
       fgs_sweeps(ab, v.Ch, v.Cv, v.D, 2 * rows, src, h, w, v.lambda, 0.25f, 3, s);
     }
     launch_lab_to_rgb8(v.sL + slot + k0.sl0, src, ab, rgb + k0.srgb0, rows, h, w, inv, s);
+    if (v.out_i420) launch_rgb8_to_i420(rgb + k0.srgb0, v.yuv + (size_t)(t & 1) * v.fp_rows * 3 / 2 + k0.srgb0 / 2, rows, h, w, s);
   }
 }
 
@@ -2125,6 +2141,7 @@ static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int
       fgs_sweeps(v.abL, v.Ch, v.Cv, v.D, R * 2, src, v.Ho, v.Wo, v.lambda, 0.25f, 3, c->sP);
     }
     launch_lab_to_rgb8(Lfull, src, v.abL, rgb, R, v.Ho, v.Wo, inv, c->sP);  // test.py:116-119
+    if (v.out_i420) launch_rgb8_to_i420(rgb, v.yuv + (size_t)(t & 1) * R * hw * 3 / 2, R, v.Ho, v.Wo, c->sP);
   }
   if (v.jpeg) {  // test.py:120 writes JPEG files: encoded here, each file stored into its slot by the encoder's last launch
     const unsigned char* slot = v.source ? v.srgb + (size_t)(t & 1) * v.fp_rows * 3 : rgb;
@@ -2138,6 +2155,15 @@ static int video_post(dvc_ctx* c, const VideoIO& v, int t, const float* abt, int
   CUDA_TRY(c, cudaStreamWaitEvent(c->sD, c->evP[t & 3], 0));
   if (v.jpeg) {
     // nothing to download: the files are in place when evP[t & 3] fires
+  } else if (v.out_i420) {  // I420 frames of 1.5 bytes per pixel, laid out like the sRGB slots they were converted from
+    const size_t rgb_slot = v.source ? v.fp_rows * 3 : (size_t)R * hw * 3;  // bytes of one sRGB slot
+    const unsigned char* yuv = v.yuv + (size_t)(t & 1) * rgb_slot / 2;
+    for (const VideoSrc& k : v.clips) {
+      const size_t n = (v.source ? (size_t)k.fp[2] * k.fp[3] : hw) * 3 / 2;
+      const size_t off = v.source ? k.srgb0 / 2 : (size_t)k.row0 * n;
+      for (int r = 0; r < k.rows; ++r)
+        CUDA_TRY(c, cudaMemcpyAsync(k.out + ((size_t)r * F + t) * n, yuv + off + r * n, n, cudaMemcpyDefault, c->sD));
+    }
   } else if (v.source) {
     const unsigned char* srgb = v.srgb + (size_t)(t & 1) * v.fp_rows * 3;
     for (const VideoSrc& k : v.clips) {
@@ -2314,15 +2340,19 @@ extern "C" int dvc_colorize_clips_exemplars(dvc_ctx* c, const float* L_in, int F
 
 // One frame source of the video calls: geometry g = (Hs, Ws, Hr, Wr, oy, ox) checked as dvc_colorize_video_rgb8 documents
 // it, then appended to v with its anti-aliasing taps
-static int video_add_source(dvc_ctx* c, const char* what, VideoIO& v, const unsigned char* frames, const int g[6], int C = 3) {
+static int video_add_source(dvc_ctx* c, const char* what, VideoIO& v, const unsigned char* frames, const int g[6],
+                            SrcFormat fmt = SrcFormat::RGB8) {
   const int Hs = g[0], Ws = g[1], Hr = g[2], Wr = g[3], oy = g[4], ox = g[5];
   if (Hs < 1 || Ws < 1 || Hr < 1 || Wr < 1 || v.Ho < 2 || v.Wo < 2 || (v.Ho & 1) || (v.Wo & 1))
     return fail(c, DVC_ERR_SHAPE, std::string(what) + ": bad geometry (sizes >= 1, an even output size)");
+  if (fmt == SrcFormat::I420 && ((Hs & 1) || (Ws & 1)))
+    return fail(c, DVC_ERR_SHAPE, std::string(what) + ": I420 frames need an even height and width");
   // the output window and the resized image nest in one another along each axis: a crop of it, or a zero pad around it
   auto nested = [](int resized, int outsz, int off) { return resized >= outsz ? off >= 0 && off <= resized - outsz : off <= 0 && off >= resized - outsz; };
   if (!nested(Hr, v.Ho, oy) || !nested(Wr, v.Wo, ox)) return fail(c, DVC_ERR_SHAPE, std::string(what) + ": crop offset outside the resized image");
   VideoSrc k;
-  k.frames = frames, k.C = C, k.Hs = Hs, k.Ws = Ws, k.Hr = Hr, k.Wr = Wr, k.oy = oy, k.ox = ox;
+  const int C = fmt == SrcFormat::GRAY8 ? 1 : 3;
+  k.frames = frames, k.fmt = fmt, k.C = C, k.Hs = Hs, k.Ws = Ws, k.Hr = Hr, k.Wr = Wr, k.oy = oy, k.ox = ox;
   std::vector<double> wy, wx;
   resize_taps(Hs, Ws, Hr, Wr, &wy, &k.ry, &wx, &k.rx);
   k.ny = (int)wy.size(), k.nx = (int)wx.size();
@@ -2330,9 +2360,11 @@ static int video_add_source(dvc_ctx* c, const char* what, VideoIO& v, const unsi
   v.taps.insert(v.taps.end(), wy.begin(), wy.end());
   v.taps.insert(v.taps.end(), wx.begin(), wx.end());
   v.taps.push_back(1.0);
-  const size_t ns = (size_t)Hs * Ws * C;
+  const size_t ns = (size_t)Hs * Ws * C;  // samples of the resize planes; an I420 frame uploads half of that
+  k.ns = fmt == SrcFormat::I420 ? ns / 2 : ns;
   k.src0 = v.ns_sum;
-  v.ns_sum += ns, v.ns_max = std::max(v.ns_max, ns);
+  v.ns_sum += k.ns, v.ns_max = std::max(v.ns_max, ns);
+  if (fmt == SrcFormat::I420) v.stage_max = std::max(v.stage_max, ns);
   v.clips.push_back(k);
   return DVC_OK;
 }
@@ -2431,8 +2463,9 @@ extern "C" int dvc_colorize_video_rgb8(dvc_ctx* c, const unsigned char* frames, 
                             stream, &v);
 }
 
-// S clips, clip s with K[s] exemplar rows (K == nullptr: one each), every clip with its own geometry and C channels per pixel.
-// The output is `out` at the window size, clip s's own window_out[s] or source_out[s] at its footprint size (K given for both).
+// S clips, clip s with K[s] exemplar rows (K == nullptr: one each), every clip with its own geometry, all in one source format.
+// The output is `out` at the window size, clip s's own window_out[s] or source_out[s] at its footprint size (K given for both),
+// as sRGB or, with out_i420, as I420 frames.
 struct JpegOut {  // dvc_colorize_videos_jpeg's destination
   int quality;
   unsigned char* const* out;
@@ -2444,7 +2477,8 @@ static int video_jpeg_outputs(dvc_ctx* c, const char* what, VideoIO& v, const in
 static int videos_impl(dvc_ctx* c, const char* what, int S, const int* K, const unsigned char* const* frames, int F, const int* geom,
                        int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
                        unsigned char* out, float* last_lab_out, void* stream, unsigned char* const* source_out = nullptr,
-                       const JpegOut* jpeg = nullptr, int C = 3, unsigned char* const* window_out = nullptr) {
+                       const JpegOut* jpeg = nullptr, SrcFormat fmt = SrcFormat::RGB8, unsigned char* const* window_out = nullptr,
+                       bool out_i420 = false) {
   if (!c || !frames || !geom || (!out && !source_out && !jpeg && !window_out) || F < 1)
     return c ? fail(c, DVC_ERR_ARG, std::string(what) + ": bad argument") : DVC_ERR_ARG;
   const int* counts = K;
@@ -2458,11 +2492,18 @@ static int videos_impl(dvc_ctx* c, const char* what, int S, const int* K, const 
   v.Ho = Ho, v.Wo = Wo;
   for (int s = 0; s < S; ++s) {
     if (!frames[s]) return fail(c, DVC_ERR_ARG, std::string(what) + ": frames[" + std::to_string(s) + "] is null");
-    DVC_TRY(video_add_source(c, what, v, frames[s], geom + 6 * s, C));
+    DVC_TRY(video_add_source(c, what, v, frames[s], geom + 6 * s, fmt));
   }
   DVC_TRY(video_finish(c, what, v, wls, wls_lambda, wls_sigma, out, last_lab_out));
   if (window_out) DVC_TRY(video_window_outputs(c, what, v, counts, window_out));
   if (source_out) DVC_TRY(video_source_outputs(c, what, v, counts, source_out));
+  if (out_i420) {
+    for (size_t s = 0; s < v.clips.size(); ++s)
+      if (v.source && ((v.clips[s].fp[2] & 1) || (v.clips[s].fp[3] & 1)))
+        return fail(c, DVC_ERR_SHAPE, std::string(what) + ": I420 output needs an even footprint, and clip " + std::to_string(s) +
+                                          "'s is " + std::to_string(v.clips[s].fp[2]) + " x " + std::to_string(v.clips[s].fp[3]));
+    v.out_i420 = true;
+  }
   if (jpeg) DVC_TRY(video_jpeg_outputs(c, what, v, counts, F, *jpeg));
   return colorize_clip_impl(c, what, nullptr, F, Ho / 2, Wo / 2, temperature, first_last_lab, S, K, nullptr, stream, &v);
 }
@@ -2594,12 +2635,28 @@ extern "C" int dvc_colorize_videos_gray8(dvc_ctx* c, int S, const int* K, const 
   if (quality == 0) {  // sRGB frames
     if (c && (stride != 0 || sizes)) return fail(c, DVC_ERR_ARG, std::string(what) + ": sRGB output (quality 0) takes stride 0 and no sizes");
     return videos_impl(c, what, S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda, wls_sigma, nullptr,
-                       last_lab_out, stream, source_resolution ? out : nullptr, nullptr, 1, source_resolution ? nullptr : out);
+                       last_lab_out, stream, source_resolution ? out : nullptr, nullptr, SrcFormat::GRAY8,
+                       source_resolution ? nullptr : out);
   }
   if (c && !sizes) return fail(c, DVC_ERR_ARG, std::string(what) + ": sizes is null");
   const JpegOut j{quality, out, stride, sizes};
   return videos_impl(c, what, S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda, wls_sigma, nullptr,
-                     last_lab_out, stream, source_resolution ? out : nullptr, &j, 1);
+                     last_lab_out, stream, source_resolution ? out : nullptr, &j, SrcFormat::GRAY8);
+}
+
+// I420 sources and, with out_i420, I420 output: the video calls with 1.5 bytes per pixel uploaded, converted to sRGB on the
+// ingest stream, and (out_i420) the sRGB output converted back on the post-processing stream before 1.5 bytes per pixel go down
+extern "C" int dvc_colorize_videos_i420(dvc_ctx* c, int S, const int* K, const unsigned char* const* frames, int F, const int* geom,
+                                        int Ho, int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda,
+                                        float wls_sigma, int source_resolution, int out_i420, unsigned char* const* out,
+                                        float* last_lab_out, void* stream) {
+  const char* what = "colorize_videos_i420";
+  if (c && !K) return fail(c, DVC_ERR_ARG, std::string(what) + ": K is null");
+  if (c && !out) return fail(c, DVC_ERR_ARG, std::string(what) + ": out is null");
+  if (c && out_i420 != 0 && out_i420 != 1) return fail(c, DVC_ERR_ARG, std::string(what) + ": out_i420 must be 0 or 1");
+  return videos_impl(c, what, S, K, frames, F, geom, Ho, Wo, temperature, first_last_lab, wls, wls_lambda, wls_sigma, nullptr,
+                     last_lab_out, stream, source_resolution ? out : nullptr, nullptr, SrcFormat::I420, source_resolution ? nullptr : out,
+                     out_i420 == 1);
 }
 
 extern "C" int dvc_encode_jpeg(dvc_ctx* c, const unsigned char* dev_rgb, int B, int H, int W, int quality, unsigned char* out,
@@ -2670,6 +2727,22 @@ extern "C" int dvc_lab_to_rgb8(dvc_ctx* c, const float* dev_l, const float* dev_
   rgb_from_xyz(inv);
   launch_lab_to_rgb8(dev_l, PlaneSrc::identity(), dev_ab, dev_rgb, B, H, W, inv, (cudaStream_t)stream);
   return check_launch(c, "lab_to_rgb8");
+}
+
+extern "C" int dvc_i420_to_rgb8(dvc_ctx* c, const unsigned char* dev_yuv, int B, int H, int W, unsigned char* dev_rgb, void* stream) {
+  if (!c || !dev_yuv || !dev_rgb || B < 1) return c ? fail(c, DVC_ERR_ARG, "i420_to_rgb8: bad argument") : DVC_ERR_ARG;
+  if (H < 2 || W < 2 || (H & 1) || (W & 1)) return fail(c, DVC_ERR_SHAPE, "i420_to_rgb8: H and W must be even");
+  CUDA_TRY(c, cudaSetDevice(c->device));
+  launch_i420_to_rgb8(dev_yuv, dev_rgb, B, H, W, (cudaStream_t)stream);
+  return check_launch(c, "i420_to_rgb8");
+}
+
+extern "C" int dvc_rgb8_to_i420(dvc_ctx* c, const unsigned char* dev_rgb, int B, int H, int W, unsigned char* dev_yuv, void* stream) {
+  if (!c || !dev_rgb || !dev_yuv || B < 1) return c ? fail(c, DVC_ERR_ARG, "rgb8_to_i420: bad argument") : DVC_ERR_ARG;
+  if (H < 2 || W < 2 || (H & 1) || (W & 1)) return fail(c, DVC_ERR_SHAPE, "rgb8_to_i420: H and W must be even");
+  CUDA_TRY(c, cudaSetDevice(c->device));
+  launch_rgb8_to_i420(dev_rgb, dev_yuv, B, H, W, (cudaStream_t)stream);
+  return check_launch(c, "rgb8_to_i420");
 }
 
 extern "C" int dvc_rgb8_to_lab(dvc_ctx* c, const unsigned char* dev_rgb, int B, int H, int W, float* dev_lab, void* stream) {

@@ -313,6 +313,10 @@ void launch_gauss_axis_f64(const double* src, double* dst, const double* w, int 
 // [Hs][Ws][C] float64 (C = 1 or 3) -> [Ho][Wo][C] uint8
 void launch_zoom_crop(const double* src, int C, int Hs, int Ws, int Hr, int Wr, int oy, int ox, unsigned char* dst, int Ho, int Wo,
                       cudaStream_t s);
+// cv2.cvtColor's BT.601 limited-range 4:2:0 conversions, bit for bit (H, W even): I420 [B][3H/2][W] (Y, then U, then V planes)
+// -> sRGB [B][H][W][3] (COLOR_YUV2RGB_I420), and sRGB -> I420 (COLOR_RGB2YUV_I420: chroma of each 2 x 2 block's top-left pixel)
+void launch_i420_to_rgb8(const unsigned char* yuv, unsigned char* rgb, int B, int H, int W, cudaStream_t s);
+void launch_rgb8_to_i420(const unsigned char* rgb, unsigned char* yuv, int B, int H, int W, cudaStream_t s);
 
 // Baseline JPEG encoder (jpeg.cu).  Header bytes (SOI .. SOS, identical for every size and quality) and the worst-case bits of
 // one 8x8 block: DC code <= 11 + value 11 bits, 63 AC coefficients of <= 16 + 10 bits (include/dvc.h: dvc_jpeg_max_bytes).

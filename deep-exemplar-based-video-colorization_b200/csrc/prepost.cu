@@ -382,6 +382,68 @@ __global__ void __launch_bounds__(256) ctx_loss_kernel(const float* __restrict__
   if (threadIdx.x == 0) loss[blockIdx.x] = (float)(-log(red[0] / N));
 }
 
+// ------------------------------------------------------------------------------------------------ I420 <-> sRGB
+// OpenCV's BT.601 limited-range 4:2:0 conversions (cv2.cvtColor COLOR_YUV2RGB_I420 / COLOR_RGB2YUV_I420, modules/imgproc
+// color_yuv.simd.hpp): fixed point with 20 fraction bits, rounding by + 2^19, arithmetic >> 20, saturation to [0, 255].  Every
+// intermediate fits in int32, so the bytes do not depend on the compiler's contraction choices.  An I420 frame [3H/2][W] is the Y
+// plane [H][W], then U [H/2][W/2], then V [H/2][W/2]; H and W are even.  One thread per 2 x 2 block of pixels, which shares one
+// (u, v): nearest-neighbour chroma in both directions (the chroma siting is not modelled).
+constexpr int kYuvShift = 20, kYuvHalf = 1 << (kYuvShift - 1);
+constexpr int kY2Rgb = 1220542, kV2R = 1673527, kV2G = -852492, kU2G = -409993, kU2B = 2116026;
+constexpr int kR2Y = 269484, kG2Y = 528482, kB2Y = 102760;
+constexpr int kR2U = -155188, kG2U = -305135, kB2U = 460324, kR2V = 460324, kG2V = -385875, kB2V = -74448;
+
+__device__ __forceinline__ unsigned char sat_u8(int v) { return (unsigned char)min(max(v, 0), 255); }
+
+// yuv [B][3H/2][W] -> rgb [B][H][W][3]
+__global__ void __launch_bounds__(256) i420_to_rgb8_kernel(const unsigned char* __restrict__ yuv, unsigned char* __restrict__ rgb, int B,
+                                                           int H, int W) {
+  const int h2 = H / 2, w2 = W / 2;
+  const size_t nb = (size_t)h2 * w2, frame = (size_t)H * W;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)B * nb; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t b = i / nb, q = i - b * nb;
+    const int by = (int)(q / w2), bx = (int)(q - (size_t)by * w2);
+    const unsigned char* Y = yuv + b * (frame * 3 / 2);
+    const int d = (int)__ldg(Y + frame + q) - 128, e = (int)__ldg(Y + frame + nb + q) - 128;
+    const int r = kYuvHalf + kV2R * e, g = kYuvHalf + kV2G * e + kU2G * d, bl = kYuvHalf + kU2B * d;
+    unsigned char* out = rgb + (b * frame + (size_t)2 * by * W + 2 * bx) * 3;
+#pragma unroll
+    for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+      for (int dx = 0; dx < 2; ++dx) {
+        const int y = max(0, (int)__ldg(Y + (size_t)(2 * by + dy) * W + 2 * bx + dx) - 16) * kY2Rgb;
+        unsigned char* px = out + ((size_t)dy * W + dx) * 3;
+        px[0] = sat_u8((y + r) >> kYuvShift);
+        px[1] = sat_u8((y + g) >> kYuvShift);
+        px[2] = sat_u8((y + bl) >> kYuvShift);
+      }
+  }
+}
+
+// rgb [B][H][W][3] -> yuv [B][3H/2][W]: Y of every pixel, U and V of the top-left pixel of each 2 x 2 block (no averaging)
+__global__ void __launch_bounds__(256) rgb8_to_i420_kernel(const unsigned char* __restrict__ rgb, unsigned char* __restrict__ yuv, int B,
+                                                           int H, int W) {
+  const int h2 = H / 2, w2 = W / 2;
+  const size_t nb = (size_t)h2 * w2, frame = (size_t)H * W;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)B * nb; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t b = i / nb, q = i - b * nb;
+    const int by = (int)(q / w2), bx = (int)(q - (size_t)by * w2);
+    const unsigned char* in = rgb + (b * frame + (size_t)2 * by * W + 2 * bx) * 3;
+    unsigned char* Y = yuv + b * (frame * 3 / 2);
+#pragma unroll
+    for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+      for (int dx = 0; dx < 2; ++dx) {
+        const unsigned char* px = in + ((size_t)dy * W + dx) * 3;
+        const int v = kR2Y * __ldg(px) + kG2Y * __ldg(px + 1) + kB2Y * __ldg(px + 2) + kYuvHalf + (16 << kYuvShift);
+        Y[(size_t)(2 * by + dy) * W + 2 * bx + dx] = sat_u8(v >> kYuvShift);
+      }
+    const int r = __ldg(in), g = __ldg(in + 1), bl = __ldg(in + 2);
+    Y[frame + q] = sat_u8((kR2U * r + kG2U * g + kB2U * bl + kYuvHalf + (128 << kYuvShift)) >> kYuvShift);
+    Y[frame + nb + q] = sat_u8((kR2V * r + kG2V * g + kB2V * bl + kYuvHalf + (128 << kYuvShift)) >> kYuvShift);
+  }
+}
+
 inline int grid_for(size_t total, int threads, int cap = 132 * 16) {
   const size_t g = (total + threads - 1) / threads;
   return (int)(g < (size_t)cap ? (g ? g : 1) : cap);
@@ -460,6 +522,14 @@ void launch_zoom_crop(const double* src, int C, int Hs, int Ws, int Hr, int Wr, 
     zoom_crop_kernel<1><<<grid_for((size_t)Ho * Wo, 256), 256, 0, s>>>(src, Hs, Ws, Hr, Wr, oy, ox, dst, Ho, Wo);
   else
     zoom_crop_kernel<3><<<grid_for((size_t)Ho * Wo * 3, 256), 256, 0, s>>>(src, Hs, Ws, Hr, Wr, oy, ox, dst, Ho, Wo);
+  launch_counter_add(1);
+}
+void launch_i420_to_rgb8(const unsigned char* yuv, unsigned char* rgb, int B, int H, int W, cudaStream_t s) {
+  i420_to_rgb8_kernel<<<grid_for((size_t)B * (H / 2) * (W / 2), 256), 256, 0, s>>>(yuv, rgb, B, H, W);
+  launch_counter_add(1);
+}
+void launch_rgb8_to_i420(const unsigned char* rgb, unsigned char* yuv, int B, int H, int W, cudaStream_t s) {
+  rgb8_to_i420_kernel<<<grid_for((size_t)B * (H / 2) * (W / 2), 256), 256, 0, s>>>(rgb, yuv, B, H, W);
   launch_counter_add(1);
 }
 

@@ -33,6 +33,7 @@ EXPORTED = [
     "dvc_colorize_videos_rgb8", "dvc_colorize_frames_clips_exemplars", "dvc_colorize_clips_exemplars",
     "dvc_colorize_videos_exemplars_rgb8", "dvc_source_footprint", "dvc_ab_to_source", "dvc_colorize_videos_source_rgb8",
     "dvc_jpeg_max_bytes", "dvc_encode_jpeg", "dvc_colorize_videos_jpeg", "dvc_colorize_videos_gray8",
+    "dvc_i420_to_rgb8", "dvc_rgb8_to_i420", "dvc_colorize_videos_i420",
 ]
 
 _lib = None
@@ -103,6 +104,10 @@ def load_library():
         lib.dvc_colorize_videos_jpeg.argtypes = [c_void, c_int, P(c_int), P(c_void), c_int, P(c_int), c_int, c_int, c_float, c_void,
                                                  c_int, c_float, c_float, c_int, c_int, P(c_void), c_i64, c_void, c_void, c_void]
         lib.dvc_colorize_videos_gray8.argtypes = lib.dvc_colorize_videos_jpeg.argtypes
+        lib.dvc_i420_to_rgb8.argtypes = [c_void, c_void, c_int, c_int, c_int, c_void, c_void]
+        lib.dvc_rgb8_to_i420.argtypes = [c_void, c_void, c_int, c_int, c_int, c_void, c_void]
+        lib.dvc_colorize_videos_i420.argtypes = [c_void, c_int, P(c_int), P(c_void), c_int, P(c_int), c_int, c_int, c_float, c_void,
+                                                 c_int, c_float, c_float, c_int, c_int, P(c_void), c_void, c_void]
         lib.dvc_exemplar_pack_size.argtypes = [c_void, c_int, c_int]
         lib.dvc_exemplar_pack_size.restype = c_i64
         lib.dvc_exemplar_export.argtypes = [c_void, c_void, c_i64, c_void]
@@ -856,6 +861,92 @@ class Context:
         res = (out, sizes) if quality is not None else (out,)
         res += (last,) if return_last else ()
         return res if len(res) > 1 else res[0]
+
+    # ---- planar YUV 4:2:0 (I420): cv2's BT.601 conversions on the device, and video calls that take and give I420 frames ---------
+    def i420_to_rgb8(self, yuv):
+        """cv2.cvtColor(COLOR_YUV2RGB_I420) of a CUDA uint8 [B,3H/2,W] tensor (H, W even): uint8 [B,H,W,3]
+        (include/dvc.h: dvc_i420_to_rgb8)."""
+        if not (isinstance(yuv, torch.Tensor) and yuv.is_cuda and yuv.dtype == torch.uint8 and yuv.dim() == 3 and yuv.shape[1] % 3 == 0):
+            raise DvcError("i420_to_rgb8: expected a CUDA uint8 tensor [B,3H/2,W]")
+        yuv = yuv.contiguous()
+        B, H, W = yuv.shape[0], yuv.shape[1] * 2 // 3, yuv.shape[2]
+        out = torch.empty(B, H, W, 3, device=yuv.device, dtype=torch.uint8)
+        self._check(self.lib.dvc_i420_to_rgb8(self.h, _ptr(yuv), B, H, W, _ptr(out), _stream(yuv.device)), "dvc_i420_to_rgb8")
+        return out
+
+    def rgb8_to_i420(self, rgb):
+        """cv2.cvtColor(COLOR_RGB2YUV_I420) of a CUDA uint8 [B,H,W,3] tensor (H, W even): uint8 [B,3H/2,W]
+        (include/dvc.h: dvc_rgb8_to_i420)."""
+        if not (isinstance(rgb, torch.Tensor) and rgb.is_cuda and rgb.dtype == torch.uint8 and rgb.dim() == 4 and rgb.shape[3] == 3):
+            raise DvcError("rgb8_to_i420: expected a CUDA uint8 tensor [B,H,W,3]")
+        rgb = rgb.contiguous()
+        B, H, W, _ = rgb.shape
+        out = torch.empty(B, H * 3 // 2, W, device=rgb.device, dtype=torch.uint8)
+        self._check(self.lib.dvc_rgb8_to_i420(self.h, _ptr(rgb), B, H, W, _ptr(out), _stream(rgb.device)), "dvc_rgb8_to_i420")
+        return out
+
+    def colorize_videos_i420(self, clips, K, size, temperature=1e-10, first_last_lab=None, wls=(500.0, 4.0), source_resolution=False,
+                             out_format="rgb", out=None, return_last=False):
+        """The video calls for I420 clips (include/dvc.h: dvc_colorize_videos_i420): clips is a list of S uint8 tensors
+        [F,3Hs/2,Ws] (Hs, Ws even).  Returns a list of S tensors, clip s's [K[s],F,h,w,3] sRGB frames (out_format="rgb") or
+        [K[s],F,3h/2,w] I420 frames (out_format="i420"), (h, w) = size, or the clip's footprint (source_footprint) with
+        source_resolution.  The sRGB frames are exactly those of colorize_videos_exemplars_rgb8 (its rows split by clip) or
+        colorize_videos_source_rgb8 for the clips converted by i420_to_rgb8, the I420 frames rgb8_to_i420 of them.
+        first_last_lab and the returned last state are [R,3,size[0]/2,size[1]/2] as there.  `out`: None or such a list on the
+        side where the clips live (pinned host or device)."""
+        from dvc.prepost import centerpad_geometry
+
+        what = "colorize_videos_i420"
+        if out_format not in ("rgb", "i420"):
+            raise DvcError(f'{what}: out_format must be "rgb" or "i420"')
+        clips = list(clips)
+        if not clips or not all(isinstance(f, torch.Tensor) and f.dtype == torch.uint8 and f.dim() == 3 and f.shape[1] % 3 == 0
+                                for f in clips):
+            raise DvcError(f"{what}: expected a list of uint8 tensors [F,3Hs/2,Ws]")
+        on_device = clips[0].is_cuda
+        if any(f.is_cuda != on_device for f in clips) or len({f.shape[0] for f in clips}) != 1:
+            raise DvcError(f"{what}: the clips must have the same frame count and all live on the host or all on the device")
+        clips = [f.contiguous() for f in clips]
+        if not on_device:
+            clips = [f if f.is_pinned() else f.pin_memory() for f in clips]
+        S, F_ = len(clips), clips[0].shape[0]
+        K, ck = self._counts(K, S, what)
+        R = sum(K)
+        Ho, Wo = int(size[0]), int(size[1])
+        geom, shapes = [], []
+        for f, k in zip(clips, K):
+            Hs, Ws = f.shape[1] * 2 // 3, f.shape[2]
+            g = [Hs, Ws, *centerpad_geometry(Hs, Ws, (Ho, Wo))]
+            h, w = tuple(source_footprint(*g, Ho, Wo)[2:]) if source_resolution else (Ho, Wo)
+            geom += g
+            shapes.append((k, F_, h, w, 3) if out_format == "rgb" else (k, F_, h * 3 // 2, w))
+
+        def host_or_device(shape, dtype):
+            t = torch.empty(*shape, dtype=dtype, device=clips[0].device)
+            return t if on_device else t.pin_memory()
+
+        if out is None:
+            out = [host_or_device(shp, torch.uint8) for shp in shapes]
+        out = list(out)
+        if len(out) != S or any(o.is_cuda != on_device or o.dtype != torch.uint8 or not o.is_contiguous() or tuple(o.shape) != shp
+                                for o, shp in zip(out, shapes)):
+            layout = "[K[s],F,h_s,w_s,3]" if out_format == "rgb" else "[K[s],F,3h_s/2,w_s]"
+            raise DvcError(f"{what}: `out` must be a list of contiguous uint8 {layout} tensors on the same side as the clips")
+        fl = None
+        if first_last_lab is not None:
+            fl = first_last_lab.to(torch.float32).contiguous()
+            if tuple(fl.shape) != (R, 3, Ho // 2, Wo // 2):
+                raise DvcError(f"{what}: first_last_lab must be [R,3,H/2,W/2]")
+        last = host_or_device((R, 3, Ho // 2, Wo // 2), torch.float32) if return_last else None
+        lam, sigma = (0.0, 1.0) if wls is None else (float(wls[0]), float(wls[1]))
+        ptrs = (ctypes.c_void_p * S)(*[f.data_ptr() for f in clips])
+        optrs = (ctypes.c_void_p * S)(*[o.data_ptr() for o in out])
+        g = (ctypes.c_int * (6 * S))(*geom)
+        rc = self.lib.dvc_colorize_videos_i420(self.h, S, ck, ptrs, F_, g, Ho, Wo, float(temperature), _ptr(fl), 0 if wls is None else 1,
+                                               lam, sigma, 1 if source_resolution else 0, 1 if out_format == "i420" else 0, optrs,
+                                               _ptr(last), _stream(self.device))
+        self._check(rc, f"dvc_{what}")
+        return (out, last) if return_last else out
 
     # ---- pre / post-processing around the nets (test.py:58,71,100-102) ----------------------------------
     def resize_half(self, x):

@@ -325,6 +325,45 @@ int dvc_colorize_videos_gray8(dvc_ctx* ctx, int S, const int* K, const unsigned 
                               int source_resolution, int quality, unsigned char* const* out, int64_t stride, int64_t* sizes,
                               float* last_lab_out, void* stream);
 
+/* ---- planar YUV 4:2:0 (I420) video -----------------------------------------------------------------------------------------
+ * The pixel format of video decoders and encoders (ffmpeg -pix_fmt yuv420p, x264, NVENC).  One H x W frame (H, W even) is
+ * [3H/2,W] uint8: the Y plane [H,W], then U [H/2,W/2], then V [H/2,W/2] -- cv2's I420 layout.  The conversions are OpenCV's
+ * cv2.cvtColor COLOR_YUV2RGB_I420 / COLOR_RGB2YUV_I420, bit for bit: the BT.601 limited-range matrix (Y in [16, 235], U / V in
+ * [16, 240] nominally; bytes outside are saturated, not refused) in 20-bit fixed point, h = 1 << 19, arithmetic >> 20, sat to
+ * [0, 255]:
+ *   YUV -> RGB: Y' = max(0, y - 16) 1220542, d = u - 128, e = v - 128;  R = sat((Y' + h + 1673527 e) >> 20),
+ *               G = sat((Y' + h - 852492 e - 409993 d) >> 20),  B = sat((Y' + h + 2116026 d) >> 20)
+ *   RGB -> YUV: Y = sat((269484 R + 528482 G + 102760 B + h + (16 << 20)) >> 20) for every pixel;
+ *               U = sat((-155188 r - 305135 g + 460324 b + h + (128 << 20)) >> 20),
+ *               V = sat((460324 r - 385875 g - 74448 b + h + (128 << 20)) >> 20) from the top-left pixel (r, g, b) of each 2 x 2
+ *               block only (no averaging).
+ * Chroma is nearest-neighbour in both directions: each (u, v) serves its 2 x 2 block, whatever chroma siting a container tags
+ * (Y4M's C420jpeg / C420mpeg2 / C420paldv are all read the same way).  Sources tagged BT.709 (most HD video) are decoded with
+ * the BT.601 matrix as OpenCV does, which gives a slightly different L than an exact BT.709 decode; an encoder should tag the
+ * output BT.601 limited range (ffmpeg: -colorspace bt470bg -color_range tv). */
+
+/* dev_yuv [B,3H/2,W] (I420) -> dev_rgb [B,H,W,3] (COLOR_YUV2RGB_I420); one launch.  DVC_ERR_SHAPE for an odd or < 2 H or W. */
+int dvc_i420_to_rgb8(dvc_ctx* ctx, const unsigned char* dev_yuv, int B, int H, int W, unsigned char* dev_rgb, void* stream);
+/* dev_rgb [B,H,W,3] -> dev_yuv [B,3H/2,W] (COLOR_RGB2YUV_I420); one launch.  DVC_ERR_SHAPE for an odd or < 2 H or W. */
+int dvc_rgb8_to_i420(dvc_ctx* ctx, const unsigned char* dev_rgb, int B, int H, int W, unsigned char* dev_yuv, void* stream);
+/* The video calls for I420 sources: frames[s] is clip s's [F,3Hs_s/2,Ws_s] uint8, host-pinned or device memory; geom holds the
+ * geometry of the luma plane (Hs_s, Ws_s even); K, the rows, the recurrence, first_last_lab and last_lab_out are as in
+ * dvc_colorize_videos_exemplars_rgb8, and exemplars stay colour images (dvc_set_exemplars).
+ *   out_i420 == 0: out[s] receives clip s's sRGB frames [K[s],F,h,w,3];
+ *   out_i420 == 1: out[s] receives them as I420 frames [K[s],F,3h/2,w];
+ * (h, w) the window (Ho, Wo), or the footprint (dvc_source_footprint) when source_resolution is set.
+ * Contract: with sRGB output every output byte and last_lab_out equal what dvc_colorize_videos_exemplars_rgb8 (its rows split
+ * by clip) or dvc_colorize_videos_source_rgb8 returns for the frames converted by dvc_i420_to_rgb8; with I420 output each frame
+ * is dvc_rgb8_to_i420 of that sRGB frame.  1.5 bytes per pixel go up (and down with out_i420).  Launches per frame step: the
+ * sRGB call's plus S (one conversion per clip on the ingest stream), plus, with out_i420, one per output size (the window, or
+ * each footprint size) on the post-processing stream.  Device memory does not depend on F.  Refuses what the sRGB calls
+ * refuse, plus a null out / out[s] or out_i420 outside {0, 1} (DVC_ERR_ARG), an odd Hs or Ws, and with out_i420 a footprint of
+ * odd height or width, which CenterPad's crop can give (DVC_ERR_SHAPE), before any launch.  Synchronises `stream` before
+ * returning. */
+int dvc_colorize_videos_i420(dvc_ctx* ctx, int S, const int* K, const unsigned char* const* frames, int F, const int* geom, int Ho,
+                             int Wo, float temperature, const float* first_last_lab, int wls, float wls_lambda, float wls_sigma,
+                             int source_resolution, int out_i420, unsigned char* const* out, float* last_lab_out, void* stream);
+
 /* ---- pre / post-processing around the nets (SURVEY.md §8f row 1) ------------------------------ */
 
 /* F.interpolate(x, scale_factor=0.5, mode="bilinear") -- test.py:58,71.  dev_src [planes,H,W] (H, W even) ->

@@ -42,7 +42,8 @@ bytes and writes what the sRGB calls write for the frames converted to RGB; a ca
 the grey frames to RGB on the host.  A folder that changes between grey and colour splits its chunks there, like a change of
 size.  Output names and bytes do not depend on which path a frame took.
 
-What the reference does and this script does not: the AVI writer (folder2vid).  Image decode stays on the host (PIL), as in
+What the reference does and this script does not: the AVI writer (folder2vid); tools/colorize_y4m.py colorizes a YUV4MPEG2
+stream instead, which ffmpeg decodes from and encodes to any container.  Image decode stays on the host (PIL), as in
 the reference, and so does PNG encoding.  Without checkpoints (none ship with the reference tree) pass --seeded-weights to run the
 pipeline on the seeded random weights of dvc/synth.py (useful as a smoke run only).
 """
@@ -82,6 +83,28 @@ def save_png(img, path):
 def save_bytes(data, path):
     with open(path, "wb") as f:
         f.write(data)
+
+
+def set_weights(ctx, vgg, warp, color, seeded):
+    """The three networks' weights from checkpoint files, or the seeded random weights of dvc/synth.py where a path is missing and
+    `seeded` is set."""
+    import dvc
+    from dvc.synth import make_state_dict
+
+    for net, key, path in ((dvc.NET_VGG, "vgg", vgg), (dvc.NET_WARP, "warp", warp), (dvc.NET_COLOR, "color", color)):
+        if path:
+            ctx.set_weights(net, torch.load(path, map_location="cpu"))
+        elif seeded:
+            ctx.set_weights(net, make_state_dict(key, seed=0))
+        else:
+            raise SystemExit(f"--{key} checkpoint missing (or pass --seeded-weights)")
+
+
+def exemplars_lab(ctx, paths, size):
+    """test.py:44-46 + 57-66: CenterPad(size) + CenterCrop(size) of the exemplar image files, Lab, 1/2 resolution:
+    [K,3,size[0]/2,size[1]/2] on the device, ready for dvc_set_exemplar(s)."""
+    refs = torch.stack([ctx.centerpad_rgb8(torch.from_numpy(load_rgb8(r).copy()).cuda(), tuple(size)) for r in paths])  # [K,H,W,3]
+    return ctx.resize_half(ctx.rgb8_to_lab(refs))
 
 
 class Source:
@@ -168,28 +191,16 @@ def main():
 
     import dvc
     from dvc.prepost import centerpad_geometry
-    from dvc.synth import make_state_dict
 
     ctx = dvc.get_context(0)
     if args.fast:
         ctx.set_math(conv=dvc.MATH_FP16X1)
-    for net, key, path in ((dvc.NET_VGG, "vgg", args.vgg), (dvc.NET_WARP, "warp", args.warp), (dvc.NET_COLOR, "color", args.color)):
-        if path:
-            ctx.set_weights(net, torch.load(path, map_location="cpu"))
-        elif args.seeded_weights:
-            ctx.set_weights(net, make_state_dict(key, seed=0))
-        else:
-            raise SystemExit(f"--{key} checkpoint missing (or pass --seeded-weights)")
+    set_weights(ctx, args.vgg, args.warp, args.color, args.seeded_weights)
 
     H, W = args.image_size
     if H % 16 or W % 32:
         raise SystemExit("--image-size must have H % 16 == 0 and W % 32 == 0 (the networks run at half of it)")
-    # test.py:44-46 + 57-66: CenterPad(image_size) + CenterCrop(image_size) of the exemplar(s), Lab, 1/2, features once
-    def exemplars_lab(paths):  # [K,3,H/2,W/2]
-        refs = torch.stack([ctx.centerpad_rgb8(torch.from_numpy(load_rgb8(r).copy()).cuda(), (H, W)) for r in paths])  # [K,H,W,3]
-        return ctx.resize_half(ctx.rgb8_to_lab(refs))
-
-    ref_lab = [exemplars_lab(p) for p in ref_paths]  # per clip
+    ref_lab = [exemplars_lab(ctx, p, (H, W)) for p in ref_paths]  # per clip; the exemplar features are computed once
 
     def stem(path):
         return os.path.splitext(os.path.basename(path))[0]
