@@ -1861,12 +1861,39 @@ static int clip_streams(dvc_ctx* c) {
 }
 
 // ---- host-side constants of the pre / post-processing kernels ---------------------------------------------------------
-static void gaussian_taps(double sigma, std::vector<double>* w, int* radius) {  // scipy.ndimage._gaussian_kernel1d, truncate = 4
+// numpy.sum of n contiguous doubles (pairwise_sum of numpy's loops_utils.h): sequential below 8 elements, else 8 running
+// sums over blocks of 8 combined as a tree plus a sequential tail, halves (rounded down to a multiple of 8) above 128.
+static double numpy_pairwise_sum(const double* a, size_t n) {
+  if (n < 8) {
+    double res = 0.0;
+    for (size_t i = 0; i < n; ++i) res += a[i];
+    return res;
+  }
+  if (n <= 128) {
+    double r[8];
+    for (int j = 0; j < 8; ++j) r[j] = a[j];
+    size_t i = 8;
+    for (; i < n - (n % 8); i += 8)
+      for (int j = 0; j < 8; ++j) r[j] += a[i + j];
+    double res = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
+    for (; i < n; ++i) res += a[i];
+    return res;
+  }
+  size_t n2 = n / 2;
+  n2 -= n2 % 8;
+  return numpy_pairwise_sum(a, n2) + numpy_pairwise_sum(a + n2, n - n2);
+}
+
+// scipy.ndimage._gaussian_kernel1d, truncate = 4: phi = exp(-0.5 / sigma^2 * x^2); phi / phi.sum().  The sum is numpy's, in
+// numpy's order: a left-to-right sum differs from it in the last bit from radius 5 up, and the truncation to uint8 sees that
+// bit wherever the filtered value sits on an integer (flat areas).  exp is libm's; numpy's own vectorised exp, where the CPU
+// has one, may differ from it in the last bit of some taps (see the header of prepost.cu).
+static void gaussian_taps(double sigma, std::vector<double>* w, int* radius) {
   const int r = (int)(4.0 * sigma + 0.5);
   w->assign(2 * r + 1, 0.0);
   const double s2 = sigma * sigma;
-  double sum = 0.0;
-  for (int x = -r; x <= r; ++x) (*w)[x + r] = exp(-0.5 / s2 * (double)(x * x)), sum += (*w)[x + r];
+  for (int x = -r; x <= r; ++x) (*w)[x + r] = exp(-0.5 / s2 * (double)(x * x));
+  const double sum = numpy_pairwise_sum(w->data(), w->size());
   for (double& v : *w) v /= sum;
   *radius = r;
 }
@@ -1879,6 +1906,19 @@ static void resize_taps(int Hs, int Ws, int Hr, int Wr, std::vector<double>* wy,
   *ry = *rx = 0;
   if (sy > 1e-15) gaussian_taps(sy, wy, ry);
   if (sx > 1e-15) gaussian_taps(sx, wx, rx);
+}
+
+// Host only (no context, no device): the taps resize_taps gives one axis, so that a test can hold them against scipy's
+extern "C" int dvc_debug_resize_taps(int in_len, int out_len, double* taps, int capacity, int* radius) {
+  if (in_len < 1 || out_len < 1 || !radius || capacity < 0 || (capacity > 0 && !taps)) return DVC_ERR_ARG;
+  if ((double)in_len / out_len > 65536.0) return DVC_ERR_SHAPE;  // keeps the tap count far inside an int
+  std::vector<double> wy, wx;
+  int ry = 0, rx = 0;
+  resize_taps(in_len, 1, out_len, 1, &wy, &ry, &wx, &rx);
+  *radius = ry;
+  if (wy.size() > (size_t)capacity) return DVC_ERR_SHAPE;
+  for (size_t i = 0; i < wy.size(); ++i) taps[i] = wy[i];
+  return DVC_OK;
 }
 
 // FGS weights_LUT[d] = -exp(-d / sigma_color), d = |difference of neighbouring guide pixels|: evaluated in double and
@@ -2706,6 +2746,8 @@ extern "C" int dvc_ab_to_source(dvc_ctx* c, const float* dev_ab, int planes, int
 extern "C" int dvc_resize_half(dvc_ctx* c, const float* dev_src, int planes, int H, int W, float* dev_dst, void* stream) {
   if (!c || !dev_src || !dev_dst || planes < 1) return c ? fail(c, DVC_ERR_ARG, "resize_half: bad argument") : DVC_ERR_ARG;
   if (H < 2 || W < 2 || (H & 1) || (W & 1)) return fail(c, DVC_ERR_SHAPE, "resize_half: H and W must be even");
+  // the kernel reads pairs of floats as one 8-byte load; with W even every pair is aligned when the first one is
+  if ((uintptr_t)dev_src & 7) return fail(c, DVC_ERR_ARG, "resize_half: dev_src must be 8-byte aligned");
   CUDA_TRY(c, cudaSetDevice(c->device));
   launch_resize_half(dev_src, dev_dst, planes, H, W, (cudaStream_t)stream);
   return check_launch(c, "resize_half");

@@ -571,8 +571,11 @@ __global__ void __launch_bounds__(256) resize_half_kernel(const float* __restric
     const long pl = t / h;
     const float* sp = src + (pl * H + 2 * i) * W + 2 * j;
     const float2 a = __ldg(reinterpret_cast<const float2*>(sp)), b = __ldg(reinterpret_cast<const float2*>(sp + W));
-    // torch: lambda = 0.5 on both axes: (a0*0.5 + a1*0.5) * 0.5 + (b0*0.5 + b1*0.5) * 0.5, rows first
-    dst[idx] = 0.5f * (0.5f * a.x + 0.5f * a.y) + 0.5f * (0.5f * b.x + 0.5f * b.y);
+    // torch: lambda = 0.5 on both axes: (a0*0.5 + a1*0.5) * 0.5 + (b0*0.5 + b1*0.5) * 0.5, rows first.  Spelled with
+    // intrinsics so that the bits do not depend on which products the compiler fuses (oracle/prepost_oracle.py states the
+    // same sequence); halving is exact except on subnormals, the only inputs on which the fused form shows.
+    const float ra = __fmaf_rn(a.x, 0.5f, __fmul_rn(a.y, 0.5f)), rb = __fmaf_rn(b.x, 0.5f, __fmul_rn(b.y, 0.5f));
+    dst[idx] = __fmaf_rn(ra, 0.5f, __fmul_rn(rb, 0.5f));
   }
 }
 
@@ -596,8 +599,12 @@ __global__ void __launch_bounds__(256) upsample2_kernel(const float* __restrict_
     const float* sp = src + pl * h * w;
     const float v00 = __ldg(sp + (long)y0 * w + x0), v01 = __ldg(sp + (long)y0 * w + x1);
     const float v10 = __ldg(sp + (long)y1 * w + x0), v11 = __ldg(sp + (long)y1 * w + x1);
-    const float v = (1.f - ly) * ((1.f - lx) * v00 + lx * v01) + ly * ((1.f - lx) * v10 + lx * v11);
-    dst[idx] = v * scale;
+    // (1 - ly) * ((1 - lx) * v00 + lx * v01) + ly * ((1 - lx) * v10 + lx * v11), then * scale: one product of every sum is
+    // fused into the addition.  Which one is spelled out (the choice the compiler made when this was plain arithmetic, so
+    // these are the bits every caller has always seen) and restated by oracle/prepost_oracle.py: upsample2_scaled_f32.
+    const float wy = __fsub_rn(1.f, ly), wx = __fsub_rn(1.f, lx);
+    const float top = __fmaf_rn(lx, v01, __fmul_rn(wx, v00)), bot = __fmaf_rn(wx, v10, __fmul_rn(lx, v11));
+    dst[idx] = __fmul_rn(__fmaf_rn(wy, top, __fmul_rn(ly, bot)), scale);
   }
 }
 

@@ -13,7 +13,14 @@
 //  * CenterPad (utils/util_distortion.py:217-258): aspect-preserving skimage.transform.resize(order=1, mode="reflect",
 //    anti_aliasing=True, preserve_range=True, clip=False) -- i.e. scipy.ndimage.gaussian_filter(sigma = (factor-1)/2,
 //    mode="mirror", truncate=4) followed by scipy.ndimage.zoom(order=1, mode="mirror", grid_mode=True), both float64 --
-//    truncation to uint8 and the centred crop / zero pad to the target size.
+//    truncation to uint8 and the centred crop / zero pad to the target size.  The taps come from the host (dvc_api.cu:
+//    gaussian_taps): summed as numpy sums them (pairwise), each exp from libm.  Reproducing numpy's own vectorised float64
+//    exp, which CPUs with AVX-512 use and which misses libm's by the last bit on some arguments, was not attempted: scipy's
+//    bytes are then not the same on every machine either.  The guarantee is therefore: scipy's bytes exactly whenever the
+//    taps agree (on the x86-64 hosts measured: every down-scale below 5x) and the source is down-scaled; else at most one level, and only where
+//    scipy's float64 value lies on an integer (flat areas).  When up-scaling, sample points before the first / after the last
+//    source pixel are split into floor and fraction and the index is mirrored, where scipy mirrors the coordinate first: the
+//    same two neighbours with weights one rounding apart (tests/test_gpu_prepost_edges.py asserts both cases).
 #include <math.h>
 #include <stdint.h>
 

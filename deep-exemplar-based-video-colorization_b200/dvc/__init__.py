@@ -33,7 +33,7 @@ EXPORTED = [
     "dvc_colorize_videos_rgb8", "dvc_colorize_frames_clips_exemplars", "dvc_colorize_clips_exemplars",
     "dvc_colorize_videos_exemplars_rgb8", "dvc_source_footprint", "dvc_ab_to_source", "dvc_colorize_videos_source_rgb8",
     "dvc_jpeg_max_bytes", "dvc_encode_jpeg", "dvc_colorize_videos_jpeg", "dvc_colorize_videos_gray8",
-    "dvc_i420_to_rgb8", "dvc_rgb8_to_i420", "dvc_colorize_videos_i420",
+    "dvc_i420_to_rgb8", "dvc_rgb8_to_i420", "dvc_colorize_videos_i420", "dvc_debug_resize_taps",
 ]
 
 _lib = None
@@ -137,6 +137,7 @@ def load_library():
         lib.dvc_debug_get_buffer.argtypes = [c_void, ctypes.c_char_p, P(c_void), P(c_i64), P(c_int)]
         lib.dvc_debug_conv2d.argtypes = [c_void, c_int, ctypes.c_char_p, c_void, c_int, c_int, c_int, c_int, c_int, c_int, c_float,
                                          c_int, c_int, c_int, c_float, c_int, c_void, c_void, c_void, c_void]
+        lib.dvc_debug_resize_taps.argtypes = [c_int, c_int, P(ctypes.c_double), c_int, P(c_int)]
         _lib = lib
         return lib
 
@@ -952,6 +953,8 @@ class Context:
     def resize_half(self, x):
         """F.interpolate(x, scale_factor=0.5, mode="bilinear") for a CUDA [B,C,H,W] tensor with even H, W."""
         x = _dev_f32(x, "resize_half input")
+        if x.data_ptr() % 8:  # a view at an odd float offset: dvc_resize_half loads pairs of floats and refuses it
+            x = x.clone()
         B, C, H, W = x.shape
         out = torch.empty(B, C, H // 2, W // 2, device=x.device, dtype=torch.float32)
         self._check(self.lib.dvc_resize_half(self.h, _ptr(x), B * C, H, W, _ptr(out), _stream(x.device)), "dvc_resize_half")
@@ -1182,6 +1185,20 @@ def source_footprint(Hs, Ws, Hr, Wr, oy, ox, Ho, Wo):
         raise DvcError(f"dvc_source_footprint failed ({rc}): geometry {(Hs, Ws, Hr, Wr, oy, ox)} has no source pixel inside the "
                        f"{Ho}x{Wo} window, or a size < 1")
     return tuple(fp)
+
+
+def resize_taps(in_len, out_len):
+    """The Gaussian taps CenterPad's anti-aliasing filter gives an axis resized from in_len to out_len pixels, as the host code
+    hands them to the kernel (dvc_debug_resize_taps; needs no GPU): a list of 2 * radius + 1 floats, empty without a filter."""
+    lib = load_library()
+    radius = ctypes.c_int(0)
+    rc = lib.dvc_debug_resize_taps(int(in_len), int(out_len), None, 0, ctypes.byref(radius))  # -2: radius set, taps do not fit
+    buf = (ctypes.c_double * (2 * radius.value + 1 if rc == -2 else 0))()
+    if rc == -2:
+        rc = lib.dvc_debug_resize_taps(int(in_len), int(out_len), buf, len(buf), ctypes.byref(radius))
+    if rc != 0:
+        raise DvcError(f"dvc_debug_resize_taps({in_len}, {out_len}) failed ({rc})")
+    return list(buf)
 
 
 def jpeg_max_bytes(h, w):

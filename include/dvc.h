@@ -367,7 +367,8 @@ int dvc_colorize_videos_i420(dvc_ctx* ctx, int S, const int* K, const unsigned c
 /* ---- pre / post-processing around the nets (SURVEY.md §8f row 1) ------------------------------ */
 
 /* F.interpolate(x, scale_factor=0.5, mode="bilinear") -- test.py:58,71.  dev_src [planes,H,W] (H, W even) ->
- * dev_dst [planes,H/2,W/2]; planes = B*C of a contiguous NCHW tensor. */
+ * dev_dst [planes,H/2,W/2]; planes = B*C of a contiguous NCHW tensor.  dev_src must be 8-byte aligned (the kernel loads
+ * pairs of floats; any cudaMalloc / torch allocation is, a view at an odd float offset is not): DVC_ERR_ARG otherwise. */
 int dvc_resize_half(dvc_ctx* ctx, const float* dev_src, int planes, int H, int W, float* dev_dst, void* stream);
 /* F.interpolate(x, scale_factor=2, mode="bilinear") * scale -- test.py:100-102 (scale = 1.25 there).
  * dev_src [planes,h,w] -> dev_dst [planes,2h,2w]. */
@@ -477,6 +478,12 @@ int dvc_debug_get_buffer(dvc_ctx* ctx, const char* name, void** dev_ptr, int64_t
 int dvc_debug_conv2d(dvc_ctx* ctx, int net, const char* name, const float* dev_x, int B, int H, int W, int dil, int stride,
                      int act, float slope, int pad_mode, int upconv, int fuse_tail, float in_bound, int out_planes,
                      const float* dev_add, float* dev_y, double* dev_stats_out, void* stream);
+/*   dvc_debug_resize_taps: host only, no context and no device.  The normalised Gaussian taps that
+ *   dvc_resize_antialias_crop_rgb8 and the video ingest give an axis resized from in_len to out_len pixels
+ *   (scipy.ndimage._gaussian_kernel1d(sigma = (in_len / out_len - 1) / 2, 0, radius = int(4 sigma + 0.5))): *radius, and the
+ *   2 * radius + 1 taps when `capacity` holds them (DVC_ERR_SHAPE when it does not; *radius is set either way).  An axis that
+ *   is not down-scaled has no filter: radius 0 and no taps. */
+int dvc_debug_resize_taps(int in_len, int out_len, double* taps, int capacity, int* radius);
 
 #ifdef __cplusplus
 }

@@ -107,7 +107,69 @@ def l_to_guide8(l_centred):
     return np.clip(np.trunc(v), 0, 255).astype(np.uint8)
 
 
+# ------------------------------------------------------------------------------------------------ fp32 resampling
+def fma_f32(a, b, c):
+    """fmaf(a, b, c) on float32 arrays: a * b + c rounded once.  The product of two float32 is exact in float64; the float64
+    sum is rounded to odd (when inexact, to the neighbour with an odd last bit), after which the rounding to float32 is the
+    rounding of the exact value (53 >= 24 + 2 bits), subnormal results included."""
+    p = np.asarray(a, np.float32).astype(np.float64) * np.asarray(b, np.float32).astype(np.float64)
+    c = np.asarray(c, np.float32).astype(np.float64)
+    p, c = np.broadcast_arrays(p, c)
+    s = p + c
+    t = s - p
+    err = (p - (s - t)) + (c - t)                            # TwoSum: p + c = s + err exactly
+    even = (s.view(np.int64) & 1) == 0
+    s = np.where((err != 0) & even, np.nextafter(s, np.where(err > 0, np.inf, -np.inf)), s)
+    return s.astype(np.float32)
+
+
+def resize_half_f32(x):
+    """resize_half_kernel (csrc/elementwise.cu) operation by operation: x [..., H, W] float32, H and W even ->
+    [..., H/2, W/2].  Per 2 x 2 block (a = upper row, b = lower row): r = fma(r.x, 0.5, r.y * 0.5) for both rows, then
+    fma(ra, 0.5, rb * 0.5).  Halving is exact except on subnormals, so on normal values this is the plain block mean."""
+    x = np.asarray(x, np.float32)
+    h = np.float32(0.5)
+    ax, ay, bx, by = x[..., 0::2, 0::2], x[..., 0::2, 1::2], x[..., 1::2, 0::2], x[..., 1::2, 1::2]
+    ra, rb = fma_f32(ax, h, ay * h), fma_f32(bx, h, by * h)
+    return fma_f32(ra, h, rb * h)
+
+
+def upsample2_scaled_f32(x, scale=1.25):
+    """upsample2_kernel (csrc/elementwise.cu) operation by operation: x [..., h, w] float32 -> [..., 2h, 2w].  Output I samples
+    source max(0, (I + 0.5) * 0.5 - 0.5) with the upper neighbour clamped to the last row; with l the fractional part,
+    top = fma(lx, v01, (1 - lx) * v00), bot = fma(1 - lx, v10, lx * v11), out = fma(1 - ly, top, ly * bot) * scale."""
+    x = np.asarray(x, np.float32)
+    f32 = np.float32
+
+    def axis(n):
+        s = np.maximum((np.arange(2 * n, dtype=f32) + f32(0.5)) * f32(0.5) - f32(0.5), f32(0))
+        i0 = s.astype(np.int64)
+        return i0, np.minimum(i0 + 1, n - 1), (s - i0.astype(f32)).astype(f32)
+
+    y0, y1, ly = axis(x.shape[-2])
+    x0, x1, lx = axis(x.shape[-1])
+    ly = ly[:, None]
+    wy, wx = f32(1) - ly, f32(1) - lx
+    v00, v01 = x[..., y0, :][..., x0], x[..., y0, :][..., x1]
+    v10, v11 = x[..., y1, :][..., x0], x[..., y1, :][..., x1]
+    top, bot = fma_f32(lx, v01, wx * v00), fma_f32(wx, v10, lx * v11)
+    return fma_f32(wy, top, ly * bot) * f32(scale)
+
+
 # ------------------------------------------------------------------------------------------------ CenterPad
+def resize_taps_twin(in_len, out_len):
+    """Twin of the host function that feeds the resize kernel its Gaussian taps (csrc/dvc_api.cu: resize_taps for one axis):
+    scipy.ndimage._gaussian_kernel1d with libm's exp (math.exp) per tap and numpy's sum.  [] when the axis needs no filter."""
+    import math
+
+    sigma = max(0.0, (in_len / out_len - 1.0) / 2.0)
+    if not sigma > 1e-15:
+        return np.zeros(0)
+    r = int(4.0 * sigma + 0.5)
+    phi = np.array([math.exp(-0.5 / (sigma * sigma) * float(x * x)) for x in range(-r, r + 1)])
+    return phi / phi.sum()
+
+
 def skimage_resize(image, new_size):
     """skimage.transform.resize(I, new_size, mode="reflect", preserve_range=True, clip=False, anti_aliasing=True) for an
     [H, W, C] array (scikit-image >= 0.19 code path), through the scipy.ndimage calls skimage makes."""

@@ -104,7 +104,7 @@ def test_fgs_filter_vs_oracle(ctx):
         out = ctx.fgs_filter(g_dev, torch.from_numpy(src).cuda()).cpu().numpy()
         ref = P.fgs_filter(guide, src, 500.0, 4.0)
         assert np.isfinite(out).all()
-        assert np.abs(out - ref).max() <= 1e-6 * np.abs(ref).max(), np.abs(out - ref).max()
+        assert np.array_equal(out, ref), np.abs(out - ref).max()
         assert abs(out.sum() - src.sum()) < 1e-3 * np.abs(src).sum()
 
 
